@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- dual-simplex iterations/sec (and wall-to-optimal) of the B200 engine on BASELINE.json's workloads.
+"""bench.py -- dual-simplex iterations/sec (and wall-to-optimal) of the GPU engine on BASELINE.json's workloads.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload c2|c3|small]
+                  [--dump-outputs DIR]
 
 Workloads
   N = 1 (default c2): BASELINE.json configs[1] -- synthetic random LP m=10k n=100k 1% nnz, fp64, dual
@@ -16,11 +17,18 @@ Workloads
       pricing pass and the factors (rows of the nucleus inverse, rows of the eta panel) are row-sharded;
       every rank holds the same m-vectors after ONE in-place NCCL all-gather per solve / pricing pass.
       A step is half a factorization cycle (541 iterations; one refactorization per two steps).  `python bench.py --gpus 1 --workload c3` measures the
-      same workload on one GPU (profiles/ holds that line; quoted in `strong_scaling_reference`).
-  Inputs are larger than L2 (CSC copy of A >= 120 MB + factors), no L2 flush is needed.
+      same workload on one GPU: the CSC + CSR copies of A take 6.5 GB and the inverse pair of a 13 k nucleus
+      about 4 GB, well inside the 80 GB of an H100.
+  Inputs are larger than L2 (CSC copy of A >= 120 MB + factors, against 50 MB of L2 on an H100), no L2 flush
+  is needed.
 
 W warm-up steps run untimed, then exactly K steps are timed with CUDA events on the engine's stream
 (max over ranks).
+
+--dump-outputs DIR writes what the timed solve returns to its caller after its last step -- primal column
+and row solution, row duals, reduced costs, status array and objective -- as DIR/<name>.npy (float64).
+The inputs are seeded and the start basis is a committed fixture, so two builds run with the same
+arguments can be compared output for output.
 
 --impl reference times the reference's CPU implementation of the path.  coin-or/Clp cannot be built
 here (its CoinUtils dependency is absent), so the arm runs the CPU restatement in oracle/
@@ -107,7 +115,7 @@ def build_workload(name, local_rank=0):
 
 
 def workload_config(name, lp, start, cycle, world):
-    """The `config` object -- identical for the b200 arm and the reference arm of the same run."""
+    """The `config` object -- identical for the GPU arm and the reference arm of the same run."""
     si = step_iterations(name, cycle)
     step = (f"{cycle} iterations + 1 refactorization" if si == cycle
             else f"{si} iterations (1 refactorization per {cycle} iterations)")
@@ -119,11 +127,11 @@ def workload_config(name, lp, start, cycle, world):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
-         "clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.sw_power_cap,power.limit")
 
     def __init__(self, index=0):
         self.lines, self.proc, self.index = [], None, index
@@ -146,28 +154,28 @@ class ClockSampler:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
         time.sleep(0.25)
         self.proc.terminate()
-        sm, mx, reasons = [], [], set()
+        sm, mx, pl, reasons = [], [], [], set()
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         for l in self.lines:
             f = [x.strip() for x in l.split(",")]
-            if len(f) < 6:
+            if len(f) < 7:
                 continue
             try:
                 sm.append(float(f[0])); mx.append(float(f[1]))
             except ValueError:
                 continue
+            try:
+                pl.append(float(f[6]))
+            except ValueError:
+                pass
             for nm, v in zip(names, f[2:6]):
                 if v.lower().startswith("active"):
                     reasons.add(nm)
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None,
-                "samples": len(sm), "reasons": sorted(reasons)}
+                "power_limit_w": max(pl) if pl else None, "samples": len(sm), "reasons": sorted(reasons)}
 
 
-def measured_peak_gbs():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        return float(json.load(open(p))["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (copy, of measured)"
-    return 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
+HBM_PEAK_GBS = 3350.0  # NVIDIA H100 SXM data sheet (HBM3, 700 W part); a data-sheet figure, not a measured one
 
 
 def oracle_sample(lp, status, cores, warm_iters, total_iters=None, seconds=None):
@@ -335,6 +343,8 @@ def main():
     ap.add_argument("--cpu-seconds", type=float, default=20.0)
     ap.add_argument("--no-optimal", action="store_true", help="skip the solve-to-optimality leg (N=1, c2)")
     ap.add_argument("--save-status", default=None, help="write the status array after the run (fixture generation)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the solution arrays of the timed solve as DIR/<name>.npy (float64)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl != "reference" else max(args.warmup, 1)
 
@@ -420,6 +430,16 @@ def main():
     nucleus = s.nucleusSize()
     if args.save_status and rank == 0:
         np.savez_compressed(args.save_status, status=s.statusArray(), iterations=s.numberIterations())
+    if args.dump_outputs and rank == 0:
+        # what Clpb_dual hands its caller after the last timed step: 24 (n + m) bytes, 2.6 MB at C2, 13.2 MB at C3
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for key, arr in (("primal_column_solution", s.primalColumnSolution()),
+                         ("primal_row_solution", s.primalRowSolution()),
+                         ("dual_row_solution", s.dualRowSolution()),
+                         ("dual_column_solution", s.dualColumnSolution()),
+                         ("status_array", s.statusArray()),
+                         ("objective_value", [s.objectiveValue()])):
+            np.save(os.path.join(args.dump_outputs, key + ".npy"), np.asarray(arr, dtype=np.float64))
 
     result = {
         "metric": "dual_simplex_iterations_per_sec", "value": value, "unit": "iterations/s",
@@ -429,7 +449,7 @@ def main():
         "config": workload_config(name, lp, start, cycle, world),
         "timed_iterations": its, "status_after_window": st, "nucleus_size": nucleus,
         "refactorizations": s.numberRefactorizations(),
-        "clocks": clocks, "gpu_launches": int(launches),
+        "gpu": torch.cuda.get_device_name(local_rank), "clocks": clocks, "gpu_launches": int(launches),
     }
     h2d = (4 * (lp.n + 1) + 12 * lp.nnz) + (4 * (lp.m + 1) + 12 * lp.nnz) + 8 * 7 * nm + nm + 12 * lp.m
     d2h = 8 * 2 * nm + 8 * lp.m + nm + 4 * lp.m
@@ -440,15 +460,6 @@ def main():
                          "includes": "per rank: Clpb_loadProblem (pageable host arrays -> HBM), NCCL communicator set-up, "
                                      "basis hand-over, Clpb_dual for W+K steps, solution read-back; max over ranks",
                          "wall_s": wall_e2e, "iterations": s.numberIterations()}
-        ref = os.path.join(ROOT, "profiles", f"r2_bench_{name}_n1.json")
-        if os.path.exists(ref):
-            try:
-                r1 = json.load(open(ref))
-                result["strong_scaling_reference"] = {"n1_value": r1["value"], "n1_ms_per_step": r1["ms_per_step"],
-                                                      "source": f"profiles/r2_bench_{name}_n1.json (python bench.py --gpus 1 --workload {name})",
-                                                      "speedup_vs_n1": value / r1["value"] if r1["value"] else None}
-            except Exception:
-                pass
 
     if world > 1:
         # ---------------- parity of the sharded path inside the scaling run itself: a small LP of the same
@@ -491,7 +502,7 @@ def main():
         ph = p.phaseTimes()
         ns = max(1.0, ph["samples"])
         k = p.nucleusSize()
-        peak, peak_src = measured_peak_gbs()
+        peak = HBM_PEAK_GBS
         nb = max(1, int((np.asarray(status) == 1)[: lp.n].sum())) if status is not None else 0
         kern = {
             # algorithmic bytes per launch (DESIGN.md "Roofline accounting")
@@ -504,30 +515,9 @@ def main():
         dom = max(kern, key=lambda q: kern[q][1])
         b, t_ms = kern[dom]
         ach = b / (t_ms * 1e-3) / 1e9 if t_ms > 0 else 0.0
-        # DRAM bytes per launch of that kernel from the committed ncu --set full capture (same
-        # workload, same nucleus size); null when the nucleus differs from the captured one
-        traffic, traffic_src, capture = None, None, None
-        for tp in ("r2_ncu_traffic.json", "r1_ncu_traffic.json"):
-            tp = os.path.join(ROOT, "profiles", tp)
-            if not os.path.exists(tp):
-                continue
-            rec = json.load(open(tp)).get(dom)
-            if rec:
-                kc = int(rec.get("nucleus_size", 0))
-                cap = {"price": kern["price"][0], "ftran_gemv": 8.0 * kc * ((kc + 7) // 8 * 8) + 48.0 * kc,
-                       "btran_gemv": 8.0 * kc * ((kc + 7) // 8 * 8) + 16.0 * kc}[dom]
-                # reported as roofline.traffic only when this run's launches have the size of the
-                # captured one; otherwise the capture is quoted separately (traffic_capture)
-                if abs(b - cap) <= 0.005 * cap:
-                    traffic, traffic_src = rec["traffic"], rec["source"]
-                capture = {"nucleus_size": kc, "algorithmic_bytes": cap, "traffic": rec["traffic"],
-                           "traffic_over_algorithmic": rec["traffic"] / cap, "source": rec["source"]}
-                break
         result["roofline"] = {"kernel": dom, "bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s",
-                              "frac": ach / peak, "frac_of_nominal_8TBps": ach / 8000.0, "traffic": traffic,
-                              "traffic_source": traffic_src,
-                              "traffic_capture": capture,
-                              "peak_source": peak_src,
+                              "frac": ach / peak,
+                              "peak_source": "H100 SXM data sheet, 3.35 TB/s HBM3 (not measured)",
                               "bytes_per_launch": b, "ms_per_launch": t_ms, "nucleus_size": k,
                               "all": {q: {"bytes": v[0], "ms": v[1], "GBps": (v[0] / (v[1] * 1e-3) / 1e9 if v[1] > 0 else 0.0),
                                           "frac": (v[0] / (v[1] * 1e-3) / 1e9 / peak if v[1] > 0 else 0.0)}
@@ -550,9 +540,8 @@ def main():
                          "iterations": e.numberIterations()}
         del e
         # ---------------- wall-to-optimal (the other half of BASELINE.json's metric).  C2 itself approaches
-        # its planted optimum only asymptotically (-25 534 after 8.4e5 iterations / 400 s against -25 267.64,
-        # profiles/r2_fullsize.json; HiGHS serial: 1e4 iterations in 3000 s), far beyond a bench run: the
-        # line carries C2's objective after the timed window, and the wall-to-optimal of the SAME generator
+        # its planted optimum only asymptotically (more than 10^6 iterations, DESIGN.md section 11), far beyond
+        # a bench run: the line carries C2's objective after the timed window, and the wall-to-optimal of the SAME generator
         # at 3 000 x 30 000 solved from the all-slack basis through the public API (host buffers in,
         # solution out), checked against the planted optimum c^T x* the generator certifies
         result["objective_after_window"] = {"objective": s.objectiveValue(), "planted_objective": lp.known_objective,

@@ -99,7 +99,7 @@ SIGNATURES = {
 
 
 def build(force: bool = False) -> str:
-    """Compile the CUDA sources for sm_100a (nvcc cross-compiles without a GPU)."""
+    """Compile the CUDA sources for sm_90a (nvcc cross-compiles without a GPU)."""
     args = ["make", "-C", os.path.join(_HERE, "csrc"), "-j8"]
     if force:
         args.append("-B")

@@ -259,10 +259,11 @@ bool Engine::shardActive() const
 }
 
 // Refactorization interval for a nucleus of size k under the default policy: the base interval (2x the
-// reference's default), stretched when the modelled cost of a refactorization -- 2k^3 flops at the ~18
-// TFLOP/s the rank-32/128 updates reach, plus ~3.5 us per panel column -- exceeds 35 % of the modelled cost
-// of the iterations of a cycle (two passes over the explicit inverse, one over A, ~110 us of latency-bound
-// kernels, at the ~4.4 TB/s the streams reach).  Capped at 2048 and by a 2 GB eta panel.
+// reference's default), stretched when the modelled cost of a refactorization -- 2k^3 flops at 18 TFLOP/s
+// for the rank-32/128 updates, plus 3.5 us per panel column -- exceeds 35 % of the modelled cost of the
+// iterations of a cycle (two passes over the explicit inverse and one over A streamed at 4.4 TB/s, plus
+// 110 us of latency-bound kernels).  Only the ratio of the two costs matters.  Capped at 2048 and by a
+// 2 GB eta panel.
 int Engine::cycleFor(int k) const
 {
   const int base = std::max(8, std::min(2 * defaultFactorizationFrequency(), 2048));
@@ -393,6 +394,9 @@ int Engine::setupDevice()
   dWeightsTmp = dalloc<double>(m);
   dSolOld = dalloc<double>(nm);
   dDrift = dalloc<unsigned long long>(1);
+  dGoodStatus = dalloc<unsigned char>(nm);
+  dGoodPivot = dalloc<int>(m);
+  haveGoodBasis = false;
   dSrcPos = dalloc<int>(m);
   d.posToNuc = dalloc<int>(m);
   d.nucRow = dalloc<int>(m);
@@ -494,8 +498,8 @@ int Engine::setupDevice()
   if (shardActive()) {
     d.shardW = worldSize;
     // the eta panel streams 8*m*t bytes (t = updates since the last refactorization, on average half
-    // the cycle); sharding it costs one more all-gather per iteration (~50 us inside the graph, measured
-    // at C3), so it is sharded only when the average replicated pass is slower than that
+    // the cycle); sharding it costs one more all-gather per iteration (modelled as 120 us of replicated
+    // streaming at 2.8 TB/s), so it is sharded only when the average replicated pass is slower than that
     d.shardPanel = shardPanelMode >= 0 ? shardPanelMode
                                        : ((8.0 * m * (tmaxHint() / 2.0)) / 2.8e12 * (1.0 - 1.0 / worldSize) > 120e-6 ? 1 : 0);
     d.shardRank = rank;
@@ -878,6 +882,8 @@ int Engine::refresh()
         else if (e.lastPrimalDrift > 1.0e-5)
           c = std::max(8, std::min(2 * e.defaultFactorizationFrequency(), 2048));
       }
+      if (e.factorizationFrequency <= 0 && e.backtracks > 0) // after a loss of accuracy: shorter and shorter
+        c = std::max(8, std::max(8, std::min(2 * e.defaultFactorizationFrequency(), 2048)) >> e.backtracks);
       e.currentCycle = std::min(c, e.d.tmax);
     }
   } cycleUpdate{*this};
@@ -903,6 +909,35 @@ int Engine::refresh()
     CUDA_OK(cudaStreamSynchronize(stream));
     memcpy(&lastPrimalDrift, &bits, sizeof(double));
     driftMeasured = true;
+  }
+  // Loss of accuracy: the fresh factors of an ill-conditioned basis give basic values that disagree with
+  // the update recurrence by orders of magnitude (drift 1e7, where accurate cycles stay below 1e3).  As
+  // ClpSimplexDual::statusOfProblemInDual does (src/ClpSimplexDual.cpp:5231-5260), go back to the last
+  // basis whose factors were accurate, restart the steepest-edge weights and refactorize more often from
+  // here on (CycleUpdate halves the base interval per back-track).  make_dual_feasible re-derives every
+  // nonbasic value and bound from the duals, so the basic set is all that has to be restored.
+  if (measure && lastPrimalDrift > 1.0e4 && haveGoodBasis && backtracks < 8) {
+    backtracks++;
+    if (logLevel > 0)
+      fprintf(stderr, "clp_b200: it %d drift %.3g: back to the last accurate basis (%d)\n", numberIterations,
+              lastPrimalDrift, backtracks);
+    CUDA_OK(cudaMemcpyAsync(d.status, dGoodStatus, nm, cudaMemcpyDeviceToDevice, stream));
+    CUDA_OK(cudaMemcpyAsync(d.pivotVariable, dGoodPivot, sizeof(int) * m, cudaMemcpyDeviceToDevice, stream));
+    const std::vector<double> ones(m, 1.0);
+    CUDA_OK(cudaMemcpyAsync(d.weights, ones.data(), sizeof(double) * m, cudaMemcpyHostToDevice, stream));
+    CUDA_OK(cudaStreamSynchronize(stream));
+    if (refactor() != 0)
+      return -1;
+    launch_compute_duals(d, dPi, dZ, stream);
+    CUDA_OK(cudaMemsetAsync(dCounters, 0, sizeof(int) * 4, stream));
+    launch_make_dual_feasible(d, currentDualBound, dCounters, stream);
+    launch_compute_primals(d, dXn, dRhs, stream);
+    kernelLaunches += 20;
+    driftMeasured = false;
+  } else if (!measure || lastPrimalDrift <= 1.0e-5) {
+    CUDA_OK(cudaMemcpyAsync(dGoodStatus, d.status, nm, cudaMemcpyDeviceToDevice, stream));
+    CUDA_OK(cudaMemcpyAsync(dGoodPivot, d.pivotVariable, sizeof(int) * m, cudaMemcpyDeviceToDevice, stream));
+    haveGoodBasis = true;
   }
   if (logLevel > 0 && (logLevel > 1 || numberRefactorizations <= 60 || numberRefactorizations % 25 == 0)) {
     // progress line (the reference prints objective / infeasibilities at every refactorization)
@@ -1217,6 +1252,8 @@ int Engine::dual()
   if (m == 0 || n == 0)
     return trivialSolve();
   driftMeasured = false;
+  haveGoodBasis = false;
+  backtracks = 0;
   lastSolveWasHot = hotStart && deviceReady && factorsValid;
   if ((lastSolveWasHot ? hotPrepare() : startup()) != 0) {
     problemStatus = 4;

@@ -1,4 +1,4 @@
-// engine.cuh -- device-resident revised dual simplex iteration engine for B200 (sm_100a).
+// engine.cuh -- device-resident revised dual simplex iteration engine for H100 (sm_90a).
 //
 // What Clp does on the host with CoinIndexedVector / CoinFactorization per iteration
 // (ClpSimplexDual::whileIterating, /root/reference/src/ClpSimplexDual.cpp:973-2384) is done
@@ -39,6 +39,20 @@ constexpr int kPriceGroups = 4;           // independent 256-thread pipelines pe
 constexpr int kPriceMaxTilesPerCta = 1024; // descriptors staged in shared memory per CTA
 constexpr int kPriceTileAlloc = kPriceTile + 8;
 constexpr int kPriceTileCols = 8;         // columns per tile (one warp each)
+
+// SMs of the current device (132 on an H100 SXM), queried once: one process drives one device.
+// Grid-stride launches are sized in multiples of it.
+inline int device_sm_count()
+{
+  static int sms = 0;
+  if (sms <= 0) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0)
+      sms = 132;
+  }
+  return sms;
+}
 
 // stop reasons written by the device into IterState.stop
 enum : int { STOP_NONE = 0, STOP_NO_ROW = 1, STOP_NO_COLUMN = 2, STOP_INACCURATE = 3,

@@ -1,4 +1,4 @@
-// engine.hpp -- host side of the B200 dual simplex engine (C++ interface behind the C ABI).
+// engine.hpp -- host side of the H100 dual simplex engine (C++ interface behind the C ABI).
 //
 // The host keeps what ClpSimplexDual keeps on the host in the reference: the iteration
 // driver (whileIterating / statusOfProblemInDual, src/ClpSimplexDual.cpp:973,4996), the
@@ -49,8 +49,8 @@ public:
   int refreshDualsEvery = 0, refreshPrimalsEvery = 0; // experiments: recompute from scratch inside a cycle
   bool timing = false;
   bool useGraph = true;
-  // 16-bit row indices for PRICE (m <= 65535): 10 instead of 12 bytes per entry.  Measured at C2: no
-  // gain (29.2 vs 29.3 us) -- the kernel is bound by the shared-memory gathers of rho, not by HBM -- so off
+  // 16-bit row indices for PRICE (m <= 65535): 10 instead of 12 bytes per entry.  No gain at C2 -- the
+  // kernel is bound by the shared-memory gathers of rho, not by HBM -- so off
   bool priceIdx16 = false;
   bool usePriceTma = false;       // TMA-staged price kernel (default: LDG-direct kernel, 26% faster)
   // 0 = choose per basis (block-banded nucleus when it pays), 1 = always the dense nucleus inverse,
@@ -178,6 +178,12 @@ private:
   unsigned long long *dDrift = nullptr;
   double lastPrimalDrift = 0.0;          // relative, of the last refresh
   bool driftMeasured = false;
+  // basis of the last refresh whose drift showed accurate factors; refresh() goes back to it when the
+  // factors lose their accuracy (ClpSimplexDual::statusOfProblemInDual restores saveStatus_ the same way)
+  unsigned char *dGoodStatus = nullptr;
+  int *dGoodPivot = nullptr;
+  bool haveGoodBasis = false;
+  int backtracks = 0;                    // in this solve; each one halves the refactorization interval
   int currentCycle = 0;                  // refactorization interval in force (adapted from the drift)
   int *dSrcPos = nullptr, *dCounters = nullptr;
   unsigned char *dFlipFlag = nullptr;

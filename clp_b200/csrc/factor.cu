@@ -33,9 +33,9 @@ constexpr int kSlabPitch = NB + 1;       // padded row pitch in shared memory (b
 constexpr int kPanelMaxRowsPerCta = 640; // 640 rows x 33 x 8 B = 165 KB of shared memory
 
 // Monotone arrival counter (never reset inside a factorization: 'target' grows by gridDim.x per
-// barrier).  One acq_rel atomic per CTA + an acquire spin -- the formulation rowpass.cu measured at
-// ~1.5 us against ~3.5 us for fence + atomic + volatile spin + fence; with one barrier per matrix
-// column that difference is half of the panel time.
+// barrier).  One acq_rel atomic per CTA + an acquire spin -- the formulation rowpass.cu found about
+// twice as fast as fence + atomic + volatile spin + fence; with one barrier per matrix column that
+// difference is a large share of the panel time.
 __device__ __forceinline__ void grid_barrier(unsigned int *counter, unsigned int target)
 {
   __syncthreads();
@@ -182,7 +182,7 @@ __global__ void __launch_bounds__(256)
 
 // ---- the same panel on ONE thread-block cluster (16 CTAs of one GPC, distributed shared memory).
 // The per-column pivot exchange of lu_panel_coop_kernel costs a grid barrier plus two dependent L2 round
-// trips (~4 us per column, ncu launch list r2: 129 us per 32-column panel); inside a cluster the candidate
+// trips; inside a cluster the candidate
 // keys, the pivot row and the diagonal row are read straight out of the peers' shared memory and the two
 // synchronisations are hardware cluster barriers.  Panels of up to 16 x kPanelMaxRowsPerCta rows.
 constexpr int kPanelCluster = 16;
@@ -383,7 +383,7 @@ __global__ void __launch_bounds__(1024)
 // perm[1+i] = touched row, perm[1+2*NB+i] = the row its final content comes from).  The elements are
 // then moved by two fully parallel kernels through a scratch buffer -- one thread per (column, touched
 // row): gather tmp[i][c] = A[from_i][c], scatter A[row_i][c] = tmp[i][c].  (One thread per column doing
-// its 2*nb strided loads serially left the GPU idle: 93 us per call at k = 4.7k.)
+// its 2*nb strided loads serially left the GPU idle.)
 __global__ void lu_perm_kernel(const int *__restrict__ ipiv, int j0, int nb, int *__restrict__ perm)
 {
   int *rows = perm + 1, *from = perm + 1 + 2 * NB;
@@ -685,11 +685,7 @@ int dense_invert(double *A, double *X, int k, int ld, int *dIpiv, int *dPerm, in
   if (!permBuf && cudaMalloc(&permBuf, sizeof(int) * (1 + 4 * NB)) != cudaSuccess)
     return -99;
   if (!pubKey) {
-    int dev = 0;
-    cudaGetDevice(&dev); // one process drives one device
-    cudaDeviceGetAttribute(&numSMs, cudaDevAttrMultiProcessorCount, dev);
-    if (numSMs <= 0)
-      numSMs = 148;
+    numSMs = device_sm_count();
     if (cudaMalloc(&pubKey, sizeof(unsigned long long) * NB * numSMs) != cudaSuccess ||
         cudaMalloc(&pubRows, sizeof(double) * NB * numSMs * NB) != cudaSuccess ||
         cudaMalloc(&pubDiag, sizeof(double) * NB * NB) != cudaSuccess ||

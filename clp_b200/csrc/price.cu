@@ -31,10 +31,10 @@ __device__ __forceinline__ void histogram_add(const DeviceModel &d, double a, do
 // One warp per column, the matrix goes from HBM straight into registers: while a column is being
 // reduced the NEXT column of the warp (4 x 32 entries: 4-byte row indices + 8-byte values) is
 // already in flight, and the column bounds are fetched two columns ahead.  Only rho lives in
-// shared memory.  Measured on B200 (tests/microbench/iter_kernels.cu, m = 10^4, n = 10^5, 10^7
-// entries): 26.6 us = 4.5 TB/s, against 36 us for every variant that stages the CSC tiles through
-// shared memory with cp.async.bulk (TMA) -- those are bound by shared-memory wavefronts (TMA
-// writes + index/value reads + rho gathers), not by HBM.
+// shared memory.  tests/microbench/iter_kernels.cu compares it (m = 10^4, n = 10^5, 10^7 entries)
+// with the variants that stage the CSC tiles through shared memory with cp.async.bulk (TMA) --
+// those are bound by shared-memory wavefronts (TMA writes + index/value reads + rho gathers), not
+// by HBM.
 // IDX16: row indices are read from the 16-bit copy (m <= 65535): 10 instead of 12 bytes per entry.
 template <int THREADS, int CTAS, bool SMEM_RHO, bool IDX16 = false>
 __global__ void __launch_bounds__(THREADS, CTAS)
@@ -313,8 +313,8 @@ __global__ void __launch_bounds__(256) histogram_kernel(DeviceModel d)
 void launch_histogram(const DeviceModel &d, cudaStream_t s)
 {
   int blocks = (d.nm + 255) / 256;
-  if (blocks > 148 * 4)
-    blocks = 148 * 4;
+  if (blocks > device_sm_count() * 4)
+    blocks = device_sm_count() * 4;
   histogram_kernel<<<blocks, 256, 0, s>>>(d);
 }
 
@@ -337,14 +337,7 @@ void launch_price(const DeviceModel &d, int colBegin, int colEnd, bool fuseHist,
     cudaFuncSetAttribute(price_ldg_kernel<1024, 1, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
     attrSet = true;
   }
-  static int numSMs = 0;
-  if (numSMs == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&numSMs, cudaDevAttrMultiProcessorCount, dev);
-    if (numSMs <= 0)
-      numSMs = 148;
-  }
+  const int numSMs = device_sm_count();
   if (g_kernelTimers)
     cudaEventRecord(g_kernelTimers->price[0], s);
   if (d.priceTileCol != nullptr && d.numPriceTiles > 0) {
@@ -388,8 +381,8 @@ void launch_price(const DeviceModel &d, int colBegin, int colEnd, bool fuseHist,
 void launch_price_slacks(const DeviceModel &d, int colBegin, int colEnd, bool fuseHist, cudaStream_t s)
 {
   int blocks = (d.nm + 255) / 256;
-  if (blocks > 148 * 8)
-    blocks = 148 * 8;
+  if (blocks > device_sm_count() * 8)
+    blocks = device_sm_count() * 8;
   row_finalize_kernel<<<blocks, 256, 0, s>>>(d, colBegin, colEnd, fuseHist);
 }
 
@@ -713,11 +706,11 @@ __global__ void chuzc_select_kernel(DeviceModel d)
 void launch_chuzc(const DeviceModel &d, cudaStream_t s)
 {
   int blocks = (d.nm + 255) / 256;
-  if (blocks > 148 * 4)
-    blocks = 148 * 4;
+  if (blocks > device_sm_count() * 4)
+    blocks = device_sm_count() * 4;
   int blocks2 = (d.nm + 1023) / 1024;
-  if (blocks2 > 148)
-    blocks2 = 148;
+  if (blocks2 > device_sm_count())
+    blocks2 = device_sm_count();
   chuzc_scan1_kernel<<<kHistBuckets / 1024, 1024, 0, s>>>(d);
   chuzc_hist2_kernel<<<blocks2, 1024, 0, s>>>(d); // + level-2 scan in its tail
   chuzc_harris_kernel<<<blocks, 256, 0, s>>>(d);
@@ -746,8 +739,8 @@ void launch_transpose_times(const DeviceModel &d, const double *pi, double *z, d
                             cudaStream_t s)
 {
   int blocks = (d.n + 7) / 8;
-  if (blocks > 148 * 16)
-    blocks = 148 * 16;
+  if (blocks > device_sm_count() * 16)
+    blocks = device_sm_count() * 16;
   if (d.n > 0)
     transpose_times_kernel<<<blocks, 256, 0, s>>>(d, pi, z, scalar);
 }
@@ -773,8 +766,8 @@ void launch_times_rows(const DeviceModel &d, const double *x, double *y, double 
                        cudaStream_t s)
 {
   int blocks = (d.m + 7) / 8;
-  if (blocks > 148 * 16)
-    blocks = 148 * 16;
+  if (blocks > device_sm_count() * 16)
+    blocks = device_sm_count() * 16;
   times_rows_kernel<<<blocks, 256, 0, s>>>(d, x, y, scalar);
 }
 

@@ -9,7 +9,7 @@
 //
 // One CTA per SM (cooperative launch => co-resident), 1024 threads; every thread owns E entries
 // of the row and keeps (alpha, |alpha|, d~, range, flags) in registers across the phases, so the
-// row is read from memory once.  Phases are separated by grid barriers (~1-2 us each) instead of
+// row is read from memory once.  Phases are separated by grid barriers instead of
 // kernel boundaries; the small scans are done redundantly by every CTA, which saves a barrier.
 //   P0 finalize row + level-1 ratio histogram + per-segment totals      | barrier
 //   P1 crossing bucket (every CTA)  P2 level-2 histogram of that bucket | barrier
@@ -28,7 +28,7 @@ namespace clpb {
 
 // Generation barrier over all CTAs of a cooperative grid; bar[0] = arrival count, bar[1] =
 // generation.  One acq_rel atomic per CTA plus an acquire spin on the generation word (which the
-// last arriver publishes with a release store): ~1.5 us, against ~3.5 us for the fence + atomic +
+// last arriver publishes with a release store): about half the cost of the fence + atomic +
 // volatile-spin + fence formulation.  'gen' is thread 0's private copy of the current generation
 // (read once at kernel start: nobody can advance it before every CTA has arrived at barrier 1).
 __device__ __forceinline__ unsigned int ld_acquire_u32(const unsigned int *p)
@@ -591,14 +591,7 @@ int g_rowPassCtas = 0;
 
 bool launch_row_pass(const DeviceModel &d, cudaStream_t s)
 {
-  static int numSMs = 0;
-  if (numSMs == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&numSMs, cudaDevAttrMultiProcessorCount, dev);
-    if (numSMs <= 0)
-      numSMs = 148;
-  }
+  const int numSMs = device_sm_count();
   // "rowPassCtas" (A/B): fewer CTAs make the grid barriers cheaper but every thread owns more entries
   int ctas = g_rowPassCtas > 0 ? (g_rowPassCtas < numSMs ? g_rowPassCtas : numSMs) : numSMs;
   if (ctas < kHistBuckets / 1024)

@@ -48,9 +48,8 @@ __global__ void gather_nucleus_kernel(DeviceModel d, const double *__restrict__ 
 
 // y[c][i] = sum_j M[i][j] * x[c][j]   (M row-major k x ldk).  One CTA streams R consecutive rows with
 // DEPTH 16-byte loads per row in flight per thread, i.e. R*DEPTH*4 KB contiguous per row and step:
-// few, long DRAM streams (measured on B200, tests/microbench/iter_kernels.cu, k = 4682 / 5787:
-// one right-hand side R=1 DEPTH=8 33 / 45 us against 37 / 56 us for R=4 DEPTH=1; three right-hand
-// sides R=2 DEPTH=2 38 / 53 us against 43 / 60 us -- x goes through L1, so more rows per CTA pay
+// few, long DRAM streams (tests/microbench/iter_kernels.cu compares the shapes: one right-hand side
+// R=1 DEPTH=8, three right-hand sides R=2 DEPTH=2 -- x goes through L1, so more rows per CTA pay
 // once there are three of them).  outIndex != nullptr: the result is scattered,
 // out[c*ostride + outIndex[i]].
 template <int NRHS, int R, int DEPTH>
@@ -514,12 +513,12 @@ static void ftran_impl(const DeviceModel &d, double *b, bool applyEtas, bool che
   // fixed launch shapes (grid-stride kernels read k from the device-side FactorDesc)
   const int maxk = d.m;
   int gblocks = (roundUp8(maxk) + 255) / 256;
-  if (gblocks > 148)
-    gblocks = 148;
+  if (gblocks > device_sm_count())
+    gblocks = device_sm_count();
   double *xg = d.ywork + (size_t)3 * roundUp8(maxk);
   if (!pregathered) // the row pass (rowpass.cu) writes xg together with the right-hand sides
     gather_nucleus_kernel<<<gblocks, 256, 0, s>>>(d, b, m, xg, NRHS, checkState);
-  int blocks = maxk < 148 * g_gemvGridMul ? maxk : 148 * g_gemvGridMul;
+  int blocks = maxk < device_sm_count() * g_gemvGridMul ? maxk : device_sm_count() * g_gemvGridMul;
   if (g_kernelTimers && checkState)
     cudaEventRecord(g_kernelTimers->ftranGemv[0], s);
   const bool sharded = d.shardW > 1;
@@ -542,9 +541,9 @@ static void ftran_impl(const DeviceModel &d, double *b, bool applyEtas, bool che
   else if (g_gemvVariantF == 6)
     CLPB_GEMV_F(1, 2);
   else if (g_gemvVariantF == 7 && !sharded)
-    gemv_warp_rows_kernel<NRHS, 4><<<148 * g_gemvGridMul, 256, 0, s>>>(d.fd, 0, xg, y, -1, nullptr, d.st, checkState);
+    gemv_warp_rows_kernel<NRHS, 4><<<device_sm_count() * g_gemvGridMul, 256, 0, s>>>(d.fd, 0, xg, y, -1, nullptr, d.st, checkState);
   else if (g_gemvVariantF == 8 && !sharded)
-    gemv_warp_rows_kernel<NRHS, 8><<<148 * g_gemvGridMul, 256, 0, s>>>(d.fd, 0, xg, y, -1, nullptr, d.st, checkState);
+    gemv_warp_rows_kernel<NRHS, 8><<<device_sm_count() * g_gemvGridMul, 256, 0, s>>>(d.fd, 0, xg, y, -1, nullptr, d.st, checkState);
   else
     CLPB_GEMV_F(2, 2);
 #undef CLPB_GEMV_F
@@ -557,20 +556,20 @@ static void ftran_impl(const DeviceModel &d, double *b, bool applyEtas, bool che
     pfi_mu_kernel<NRHS><<<d.tmax, 256, 0, s>>>(d, checkState);
     if (sharded && d.shardPanel) {
       int pblocks = (d.shardPerM + 7) / 8;
-      if (pblocks > 148 * 8)
-        pblocks = 148 * 8;
+      if (pblocks > device_sm_count() * 8)
+        pblocks = device_sm_count() * 8;
       pfi_apply_warp_kernel<NRHS><<<pblocks, 256, 0, s>>>(d, b, m, checkState, false);
       shard_all_gather(d.gatherP, sizeof(double) * NRHS * d.shardPerM, s);
       pfi_merge_kernel<NRHS><<<(m + 255) / 256, 256, 0, s>>>(d, b, m, checkState, pivotTail);
     } else if (g_pfiApplyVariant == 1) {
       int pblocks = (m + 1) / 2;
-      if (pblocks > 148 * 8)
-        pblocks = 148 * 8;
+      if (pblocks > device_sm_count() * 8)
+        pblocks = device_sm_count() * 8;
       pfi_apply_kernel<NRHS><<<pblocks, 256, 0, s>>>(d, b, m, checkState, pivotTail);
     } else {
       int pblocks = (m + 7) / 8;
-      if (pblocks > 148 * 8)
-        pblocks = 148 * 8;
+      if (pblocks > device_sm_count() * 8)
+        pblocks = device_sm_count() * 8;
       pfi_apply_warp_kernel<NRHS><<<pblocks, 256, 0, s>>>(d, b, m, checkState, pivotTail);
     }
   }
@@ -750,15 +749,15 @@ static void btran_gemv(const DeviceModel &d, double *rhoOut, bool checkState, cu
 static void btran_tail(const DeviceModel &d, double *rhoOut, bool checkState, cudaStream_t s)
 {
   int sblocks = (d.m + 7) / 8;
-  if (sblocks > 148 * 8)
-    sblocks = 148 * 8;
+  if (sblocks > device_sm_count() * 8)
+    sblocks = device_sm_count() * 8;
   btran_s_kernel<<<sblocks, 256, 0, s>>>(d, checkState);
   btran_gemv(d, rhoOut, checkState, s);
 }
 
 static void btran_gemv(const DeviceModel &d, double *rhoOut, bool checkState, cudaStream_t s)
 {
-  int blocks = d.m < 148 * g_gemvGridMul ? d.m : 148 * g_gemvGridMul;
+  int blocks = d.m < device_sm_count() * g_gemvGridMul ? d.m : device_sm_count() * g_gemvGridMul;
   if (g_kernelTimers && checkState)
     cudaEventRecord(g_kernelTimers->btranGemv[0], s);
   const bool sharded = d.shardW > 1;
@@ -776,9 +775,9 @@ static void btran_gemv(const DeviceModel &d, double *rhoOut, bool checkState, cu
   else if (g_gemvVariantB == 5)
     CLPB_GEMV_B(4, 2);
   else if (g_gemvVariantB == 6 && !sharded)
-    gemv_warp_rows_kernel<1, 8><<<148 * g_gemvGridMul, 256, 0, s>>>(d.fd, 1, d.swork, rhoOut, d.m, d.nucRow, d.st, checkState);
+    gemv_warp_rows_kernel<1, 8><<<device_sm_count() * g_gemvGridMul, 256, 0, s>>>(d.fd, 1, d.swork, rhoOut, d.m, d.nucRow, d.st, checkState);
   else if (g_gemvVariantB == 7 && !sharded)
-    gemv_warp_rows_kernel<1, 4><<<148 * g_gemvGridMul, 256, 0, s>>>(d.fd, 1, d.swork, rhoOut, d.m, d.nucRow, d.st, checkState);
+    gemv_warp_rows_kernel<1, 4><<<device_sm_count() * g_gemvGridMul, 256, 0, s>>>(d.fd, 1, d.swork, rhoOut, d.m, d.nucRow, d.st, checkState);
   else
     CLPB_GEMV_B(1, 8);
 #undef CLPB_GEMV_B
@@ -787,7 +786,7 @@ static void btran_gemv(const DeviceModel &d, double *rhoOut, bool checkState, cu
   if (sharded) {
     shard_all_gather(d.gatherB, sizeof(double) * d.shardPerK, s);
     int sb = (d.m + 255) / 256;
-    btran_scatter_kernel<<<sb > 148 * 4 ? 148 * 4 : sb, 256, 0, s>>>(d, rhoOut, checkState);
+    btran_scatter_kernel<<<sb > device_sm_count() * 4 ? device_sm_count() * 4 : sb, 256, 0, s>>>(d, rhoOut, checkState);
   }
 }
 
@@ -797,8 +796,8 @@ void launch_btran_unit(const DeviceModel &d, bool checkState, cudaStream_t s)
   (void)checkState;
   launch_eta_rowvec(d, 0, true, s); // no-op when numEtas == 0
   int sblocks = (d.m + 7) / 8;
-  if (sblocks > 148 * 8)
-    sblocks = 148 * 8;
+  if (sblocks > device_sm_count() * 8)
+    sblocks = device_sm_count() * 8;
   btran_us_kernel<<<sblocks, 256, 0, s>>>(d, d.rho);
   btran_gemv(d, d.rho, true, s);
 }

@@ -92,8 +92,8 @@ __global__ void chuzr_finish_kernel(DeviceModel d)
 void launch_chuzr(const DeviceModel &d, cudaStream_t s)
 {
   int blocks = (d.m + 255) / 256;
-  if (blocks > 148 * 4)
-    blocks = 148 * 4;
+  if (blocks > device_sm_count() * 4)
+    blocks = device_sm_count() * 4;
   if (blocks < 32)
     blocks = 32; // also clears the ratio-test histograms
   chuzr_kernel<<<blocks, 256, 0, s>>>(d);
@@ -302,10 +302,10 @@ __global__ void __launch_bounds__(256) build_rhs3_kernel(DeviceModel d)
 void launch_dual_update_and_flips(const DeviceModel &d, unsigned int *flipBits, cudaStream_t s)
 {
   int blocks = (d.nm + 255) / 256;
-  if (blocks > 148 * 8)
-    blocks = 148 * 8;
+  if (blocks > device_sm_count() * 8)
+    blocks = device_sm_count() * 8;
   dual_update_kernel<<<blocks, 256, 0, s>>>(d, flipBits);
-  flip_scatter_kernel<<<148, 256, 0, s>>>(d);
+  flip_scatter_kernel<<<device_sm_count(), 256, 0, s>>>(d);
   build_rhs3_kernel<<<(d.m + 255) / 256, 256, 0, s>>>(d);
 }
 
@@ -725,7 +725,7 @@ __global__ void primal_drift_kernel(DeviceModel d, const double *__restrict__ xo
 void launch_primal_drift(const DeviceModel &d, const double *xold, unsigned long long *out, cudaStream_t s)
 {
   int blocks = (d.m + 255) / 256;
-  primal_drift_kernel<<<blocks > 148 * 4 ? 148 * 4 : blocks, 256, 0, s>>>(d, xold, out);
+  primal_drift_kernel<<<blocks > device_sm_count() * 4 ? device_sm_count() * 4 : blocks, 256, 0, s>>>(d, xold, out);
 }
 
 // ---- host wrappers used by engine.cu

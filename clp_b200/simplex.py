@@ -4,7 +4,7 @@ Method names, argument meaning and status codes follow ClpSimplex / ClpModel
 (/root/reference/src/ClpSimplex.hpp, ClpModel.hpp): ``loadProblem``, ``readMps``, ``dual``,
 ``status`` (0 optimal, 1 primal infeasible, 2 dual infeasible, 3 stopped, 4 errors),
 ``objectiveValue``, ``primalColumnSolution`` ... Everything computational happens behind the
-C ABI of include/clp_b200.h in hand-written sm_100a CUDA; this module only marshals arrays.
+C ABI of include/clp_b200.h in hand-written sm_90a CUDA; this module only marshals arrays.
 """
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-/* clp_b200.h -- C ABI of the B200-native revised dual simplex engine.
+/* clp_b200.h -- C ABI of the H100-native revised dual simplex engine.
  *
  * Drop-in boundary for ONE path of coin-or/Clp: ClpModel::readMps/loadProblem ->
  * ClpSimplex::dual().  Every entry point names the reference interface it replaces

@@ -44,5 +44,6 @@ for w in which:
             r["rel_diff"] = abs(r["objective"] - expect) / (1 + abs(expect))
         print(json.dumps(r), flush=True)
         out.append(r)
-os.makedirs("gpurun_out", exist_ok=True)
-json.dump(out, open(os.path.join("gpurun_out", "fullsize_probe_%s.json" % "_".join(which)), "w"), indent=1)
+outdir = os.environ.get("CLPB_PROBE_OUT", ".")
+os.makedirs(outdir, exist_ok=True)
+json.dump(out, open(os.path.join(outdir, "fullsize_probe_%s.json" % "_".join(which)), "w"), indent=1)

@@ -1,9 +1,8 @@
 """Start basis of the C3 bench window (BASELINE.json configs[2], m=50k n=500k): the basis the GPU
 engine reaches after ITER dual simplex iterations from the all-slack basis -- the analogue of
 tests/golden/c2_status_it12000.npz (which the CPU oracle produced; at C3 the oracle would need days).
-Needs a B200:   python tests/golden/make_c3_fixture.py [ITER]   -> tests/golden/c3_status.npz
-(also copied to gpurun_out/ so that it travels back from the GPU box)."""
-import os, shutil, sys, time
+Needs a GPU:   python tests/golden/make_c3_fixture.py [ITER]   -> tests/golden/c3_status.npz"""
+import os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
 import numpy as np
@@ -25,6 +24,4 @@ t = time.time(); st = s.dual(); el = time.time() - t
 print("status", st, "iterations", s.numberIterations(), "refactorizations", s.numberRefactorizations(), "nucleus", s.nucleusSize(),
       "seconds", round(el, 1), "it/s", round(s.numberIterations() / max(1e-9, s.secondsInLoop()), 1), flush=True)
 np.savez_compressed(fx, status=s.statusArray(), iterations=s.numberIterations())
-os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-shutil.copy(fx, os.path.join(ROOT, "gpurun_out", "c3_status.npz"))
 print("wrote", fx, os.path.getsize(fx), "bytes")

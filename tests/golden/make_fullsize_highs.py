@@ -1,5 +1,6 @@
 import os, sys, time, json
-sys.path.insert(0, '/root/repo'); sys.path.insert(0, '/root/repo/tests/golden')
+HERE = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, os.path.dirname(os.path.dirname(HERE))); sys.path.insert(0, HERE)
 import numpy as np
 from clp_b200 import generators as G
 from make_golden import highs_objective

@@ -5,12 +5,21 @@
 //     large tiles per CTA (u32 or u16 row indices)
 //   * rank-32 DGEMM update of the refactorization: SIMT 4x4 kernel vs. DMMA (mma.m8n8k4.f64)
 // Not part of the product; built and run by hand:
-//   nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -o ik iter_kernels.cu && ./ik
+//   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o ik iter_kernels.cu && ./ik
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>
+
+// SMs of device 0 (132 on an H100 SXM): launch shapes are multiples of it
+static int numSms()
+{
+  static int s = 0;
+  if (s == 0)
+    cudaDeviceGetAttribute(&s, cudaDevAttrMultiProcessorCount, 0);
+  return s;
+}
 #include <random>
 #include <vector>
 
@@ -916,7 +925,7 @@ int main(int argc, char **argv)
         }
         printf("k=%d %-46s %7.1f us  %7.1f GB/s  relerr %.1e\n", k, name, ms * 1000, bytes / ms / 1e6, d);
       };
-      for (int grid : {1184, 1480, 2368}) {
+      for (int grid : {8 * numSms(), 10 * numSms(), 16 * numSms()}) {
         char nm[96];
         CK(cudaMemset(out, 0, sizeof(double) * 3 * ldk));
         float t1 = timeit([&] { gemv_cur<1><<<grid, 256>>>(Mw(), k, ldk, x3, out); });
@@ -952,7 +961,7 @@ int main(int argc, char **argv)
         CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
         CK(cudaMemset(out, 0, sizeof(double) * 3 * ldk));
         float t = timeit([&] {
-          kern<<<148, threads, sm>>>(Mw(), k, ldk, b, m, gather, part, ticket, out, ldk, nullptr, Q, seg2);
+          kern<<<numSms(), threads, sm>>>(Mw(), k, ldk, b, m, gather, part, ticket, out, ldk, nullptr, Q, seg2);
         });
         char nm[96];
         snprintf(nm, 96, "%s Q=%d", name, Q);
@@ -1061,14 +1070,14 @@ int main(int argc, char **argv)
       int4 *dDesc;
       CK(cudaMalloc(&dDesc, sizeof(int) * desc.size()));
       CK(cudaMemcpy(dDesc, desc.data(), sizeof(int) * desc.size(), cudaMemcpyHostToDevice));
-      const int pipes = 148 * kPriceGroups;
+      const int pipes = numSms() * kPriceGroups;
       const int descCap = ((ntl + pipes - 1) / pipes + 7) / 8 * 8;
       const size_t smem = 128 + (size_t)kPriceGroups * descCap * 16 + (size_t)kPriceGroups * kPriceStages * kPriceTileAlloc * 12 + sizeof(double) * m;
       CK(cudaFuncSetAttribute(price_cur, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
       CK(cudaMemset(dAlpha, 0, sizeof(double) * n));
       float t = timeit([&] {
         win = (win + 1) % NW;
-        price_cur<<<148, 1024, smem>>>(dIdx + win * stride, dVal + win * stride, dCs, dRho, m, dAlpha, dDesc, ntl, descCap);
+        price_cur<<<numSms(), 1024, smem>>>(dIdx + win * stride, dVal + win * stride, dCs, dRho, m, dAlpha, dDesc, ntl, descCap);
       });
       char nm[96];
       snprintf(nm, 96, "price_cur 4x2x1024 (%d tiles, smem %zu)", ntl, smem);
@@ -1095,7 +1104,7 @@ int main(int argc, char **argv)
       c = c1;                                                                                                     \
       ntl++;                                                                                                      \
     }                                                                                                             \
-    const int descCap = ((ntl + 147) / 148 + 7) / 8 * 8;                                                          \
+    const int descCap = ((ntl + numSms() - 1) / numSms() + 7) / 8 * 8;                                                          \
     const size_t smem = 128 + (size_t)descCap * 16 + (size_t)S * (MAXC + 8) * 4 + (size_t)S * E * (8 + sizeof(IDXT)) + (SR ? sizeof(double) * m : 0); \
     char nm[128];                                                                                                 \
     snprintf(nm, 128, "price_big E=%d S=%d idx%zu rho:%s (%d tiles, smem %zu)", E, S, sizeof(IDXT) * 8, SR ? "smem" : "ldg", ntl, smem); \
@@ -1107,7 +1116,7 @@ int main(int argc, char **argv)
     CK(cudaMemset(dAlpha, 0, sizeof(double) * n));                                                                \
     float t = timeit([&] {                                                                                        \
       win = (win + 1) % NW;                                                                                       \
-      price_big<EE, SS, IDXT, SR><<<148, 1024, smem>>>(IDXPTR + win * stride, dVal + win * stride, dCs, dRho, m, dAlpha, dDesc, ntl, descCap); \
+      price_big<EE, SS, IDXT, SR><<<numSms(), 1024, smem>>>(IDXPTR + win * stride, dVal + win * stride, dCs, dRho, m, dAlpha, dDesc, ntl, descCap); \
     });                                                                                                           \
     report(nm, t, 8.0 + sizeof(IDXT));                                                                            \
     cudaFree(dDesc);                                                                                              \
@@ -1132,7 +1141,7 @@ int main(int argc, char **argv)
       c = c1;                                                                                                     \
       ntl++;                                                                                                      \
     }                                                                                                             \
-    const int descCap = ((ntl + 147) / 148 + 7) / 8 * 8;                                                          \
+    const int descCap = ((ntl + numSms() - 1) / numSms() + 7) / 8 * 8;                                                          \
     const size_t smem = 128 + (size_t)descCap * 16 + (size_t)S * (MAXC + 8) * 4 + (size_t)S * E * (8 + sizeof(IDXT)) + sizeof(double) * m; \
     char nm[160];                                                                                                 \
     snprintf(nm, 160, "price_v3 E=%d S=%d idx%zu lpc=%d thr=%d maxc=%d (%d tiles, smem %zu)", E, S, sizeof(IDXT) * 8, LPCV, THR, MAXCOLS, ntl, smem); \
@@ -1144,7 +1153,7 @@ int main(int argc, char **argv)
     CK(cudaMemset(dAlpha, 0, sizeof(double) * n));                                                                \
     float t = timeit([&] {                                                                                        \
       win = (win + 1) % NW;                                                                                       \
-      price_v3<EE, SS, IDXT, LPCV, THR><<<148, THR, smem>>>(IDXPTR + win * stride, dVal + win * stride, dCs, dRho, m, dAlpha, dDesc, ntl, descCap); \
+      price_v3<EE, SS, IDXT, LPCV, THR><<<numSms(), THR, smem>>>(IDXPTR + win * stride, dVal + win * stride, dCs, dRho, m, dAlpha, dDesc, ntl, descCap); \
     });                                                                                                           \
     report(nm, t, 8.0 + sizeof(IDXT));                                                                            \
     cudaFree(dDesc);                                                                                              \
@@ -1156,7 +1165,7 @@ int main(int argc, char **argv)
     CK(cudaMemset(dAlpha, 0, sizeof(double) * n));                                                 \
     float t = timeit([&] {                                                                         \
       win = (win + 1) % NW;                                                                        \
-      price_ldg<THR, CT><<<148 * CT, THR, sizeof(double) * m>>>(dIdx + win * stride, dVal + win * stride, dCs, dRho, m, dAlpha, n); \
+      price_ldg<THR, CT><<<numSms() * CT, THR, sizeof(double) * m>>>(dIdx + win * stride, dVal + win * stride, dCs, dRho, m, dAlpha, n); \
     });                                                                                            \
     char nm[96];                                                                                   \
     snprintf(nm, 96, "price_ldg thr=%d ctas/SM=%d", THR, CT);                                      \

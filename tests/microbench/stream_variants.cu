@@ -1,9 +1,18 @@
 // stream_variants.cu -- micro-benchmarks behind the design choices of the two HBM-streaming
 // kernels (PRICE over the CSC arrays, GEMV over the nucleus inverse).  Not part of the product;
-// built and run by hand:   nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o sv stream_variants.cu
+// built and run by hand:   nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o sv stream_variants.cu
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>
+
+// SMs of device 0 (132 on an H100 SXM): launch shapes are multiples of it
+static int numSms()
+{
+  static int s = 0;
+  if (s == 0)
+    cudaDeviceGetAttribute(&s, cudaDevAttrMultiProcessorCount, 0);
+  return s;
+}
 #include <vector>
 
 #define CK(x)                                                                                      \
@@ -401,13 +410,13 @@ int main()
   const double bytes = 12.0 * n;
   auto rep = [&](const char *name, float ms) { printf("%-46s %8.1f us  %7.1f GB/s\n", name, ms * 1000, bytes / ms / 1e6); fflush(stdout); };
 
-  rep("V0 plain LDG stream 148x8x512", timeit([&] { NEXTWIN(); v0_ldg<<<148 * 8, 512>>>(idx, val, n, out); }));
-  rep("V0 plain LDG stream 148x4x512", timeit([&] { NEXTWIN(); v0_ldg<<<148 * 4, 512>>>(idx, val, n, out); }));
+  rep("V0 plain LDG stream SMSx8x512", timeit([&] { NEXTWIN(); v0_ldg<<<numSms() * 8, 512>>>(idx, val, n, out); }));
+  rep("V0 plain LDG stream SMSx4x512", timeit([&] { NEXTWIN(); v0_ldg<<<numSms() * 4, 512>>>(idx, val, n, out); }));
 #define RUN_TMA(ST, TL, MODE, AL, NAME)                                                            \
   {                                                                                                \
     size_t sm = 128 + (size_t)ST * TL * 12 + (MODE >= 1 ? m * 8 : 0);                              \
     CK(cudaFuncSetAttribute(v_tma<ST, TL>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); \
-    rep(NAME, timeit([&] { NEXTWIN(); v_tma<ST, TL><<<148, 1024, sm>>>(idx, val, n, rho, m, out, MODE, AL); })); \
+    rep(NAME, timeit([&] { NEXTWIN(); v_tma<ST, TL><<<numSms(), 1024, sm>>>(idx, val, n, rho, m, out, MODE, AL); })); \
   }
   RUN_TMA(3, 3072, 0, 0, "TMA 3x3072 load only, 128B aligned");
   RUN_TMA(3, 3072, 0, 4, "TMA 3x3072 load only, 16B aligned");
@@ -422,7 +431,7 @@ int main()
   {
     size_t sm = (size_t)m * 8 + 2 * 2048 * 8;
     CK(cudaFuncSetAttribute(v_ldg_tile, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    rep("LDG tile 2048 (512 thr, 2 CTA/SM) full", timeit([&] { NEXTWIN(); v_ldg_tile<<<148 * 2, 512, sm>>>(idx, val, n, rho, m, out); }));
+    rep("LDG tile 2048 (512 thr, 2 CTA/SM) full", timeit([&] { NEXTWIN(); v_ldg_tile<<<numSms() * 2, 512, sm>>>(idx, val, n, rho, m, out); }));
   }
 
   {
@@ -430,16 +439,16 @@ int main()
     CK(cudaFuncSetAttribute(v_tma_split<3, 3072, 12>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     CK(cudaFuncSetAttribute(v_tma_split<6, 3072, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     size_t sm3 = 128 + 3 * 3072 * 12, sm6 = 128 + 6 * 3072 * 12;
-    rep("TMA 3x3072 load only, 4 sub-copies", timeit([&] { NEXTWIN(); v_tma_split<3, 3072, 4><<<148, 1024, sm3>>>(idx, val, n, out); }));
-    rep("TMA 3x3072 load only, 12 sub-copies", timeit([&] { NEXTWIN(); v_tma_split<3, 3072, 12><<<148, 1024, sm3>>>(idx, val, n, out); }));
-    rep("TMA 6x3072 load only, 4 sub-copies", timeit([&] { NEXTWIN(); v_tma_split<6, 3072, 4><<<148, 1024, sm6>>>(idx, val, n, out); }));
+    rep("TMA 3x3072 load only, 4 sub-copies", timeit([&] { NEXTWIN(); v_tma_split<3, 3072, 4><<<numSms(), 1024, sm3>>>(idx, val, n, out); }));
+    rep("TMA 3x3072 load only, 12 sub-copies", timeit([&] { NEXTWIN(); v_tma_split<3, 3072, 12><<<numSms(), 1024, sm3>>>(idx, val, n, out); }));
+    rep("TMA 6x3072 load only, 4 sub-copies", timeit([&] { NEXTWIN(); v_tma_split<6, 3072, 4><<<numSms(), 1024, sm6>>>(idx, val, n, out); }));
   }
   {
     size_t sm = (size_t)m * 8 + 2048 * 8;
     CK(cudaFuncSetAttribute(v_ldg_prefetch<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024));
     CK(cudaFuncSetAttribute(v_ldg_prefetch<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024));
-    rep("LDG prefetch 512thr 2CTA/SM load only", timeit([&] { NEXTWIN(); v_ldg_prefetch<2><<<148 * 2, 512, sm>>>(idx, val, n, rho, m, out, 0); }));
-    rep("LDG prefetch 512thr 2CTA/SM full", timeit([&] { NEXTWIN(); v_ldg_prefetch<2><<<148 * 2, 512, sm>>>(idx, val, n, rho, m, out, 1); }));
+    rep("LDG prefetch 512thr 2CTA/SM load only", timeit([&] { NEXTWIN(); v_ldg_prefetch<2><<<numSms() * 2, 512, sm>>>(idx, val, n, rho, m, out, 0); }));
+    rep("LDG prefetch 512thr 2CTA/SM full", timeit([&] { NEXTWIN(); v_ldg_prefetch<2><<<numSms() * 2, 512, sm>>>(idx, val, n, rho, m, out, 1); }));
   }
 
   // ---- GEMV: k = 4682
@@ -459,11 +468,11 @@ int main()
     CK(cudaFuncSetAttribute(gemv_warp_row_smemx<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
     CK(cudaFuncSetAttribute(gemv_warp_row_smemx<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
     size_t sm = (size_t)ldk * 8;
-    repg("GEMV warp-per-row smem x depth4 148x4x512", timeit([&] { gemv_warp_row_smemx<4><<<148 * 4, 512, sm>>>(M, k, ldk, x, out); }));
-    repg("GEMV warp-per-row smem x depth8 148x4x512", timeit([&] { gemv_warp_row_smemx<8><<<148 * 4, 512, sm>>>(M, k, ldk, x, out); }));
-    repg("GEMV warp-per-row smem x depth8 148x2x512", timeit([&] { gemv_warp_row_smemx<8><<<148 * 2, 512, sm>>>(M, k, ldk, x, out); }));
+    repg("GEMV warp-per-row smem x depth4 SMSx4x512", timeit([&] { gemv_warp_row_smemx<4><<<numSms() * 4, 512, sm>>>(M, k, ldk, x, out); }));
+    repg("GEMV warp-per-row smem x depth8 SMSx4x512", timeit([&] { gemv_warp_row_smemx<8><<<numSms() * 4, 512, sm>>>(M, k, ldk, x, out); }));
+    repg("GEMV warp-per-row smem x depth8 SMSx2x512", timeit([&] { gemv_warp_row_smemx<8><<<numSms() * 2, 512, sm>>>(M, k, ldk, x, out); }));
   }
   // plain copy-like read of M for reference
-  rep("(ref) V0 LDG stream again", timeit([&] { NEXTWIN(); v0_ldg<<<148 * 8, 512>>>(idx, val, n, out); }));
+  rep("(ref) V0 LDG stream again", timeit([&] { NEXTWIN(); v0_ldg<<<numSms() * 8, 512>>>(idx, val, n, out); }));
   return 0;
 }

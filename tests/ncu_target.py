@@ -1,5 +1,5 @@
 """Profiling target (not a test): a short mid-solve window of the C2 workload without graph
-replay, so that ncu sees ordinary kernel launches.  Used by the commands in profiles/README.md."""
+replay, so that a kernel profiler (ncu, torch.profiler) sees ordinary kernel launches."""
 import os, sys
 sys.path.insert(0, ".")
 import numpy as np

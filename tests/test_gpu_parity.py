@@ -339,7 +339,7 @@ def test_kernel_variants_take_the_same_pivots(name):
 
 
 def test_long_row_uses_multi_entry_row_pass():
-    """n+m above 148*1024: every thread of the cooperative row kernel owns two entries of the
+    """n+m above 132*1024 (one 1024-thread CTA per SM of an H100): every thread of the cooperative row kernel owns two entries of the
     tableau row (row_pass_kernel<2>); same optimum as the planted solution and as the separate
     kernels."""
     lp = G.random_sparse_lp(500, 170000, 0.02, 31)
