@@ -74,8 +74,6 @@ SIGNATURES = {
     "Clpb_times": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_double, c_double_p, c_double_p]),
     "Clpb_dualColumn": (ctypes.c_int, [ctypes.c_void_p, c_double_p, c_double_p, c_ubyte_p, ctypes.c_int,
                                        ctypes.c_double, c_double_p]),
-    "Clpb_dualColumnRowPass": (ctypes.c_int, [ctypes.c_void_p, c_double_p, c_double_p, c_ubyte_p, ctypes.c_int,
-                                              ctypes.c_double, c_double_p]),
     "Clpb_denseInvert": (ctypes.c_int, [ctypes.c_int, c_double_p, c_double_p]),
     "Clpb_pivotRow": (ctypes.c_int, [ctypes.c_void_p, c_int_p, c_int_p, c_double_p]),
     "Clpb_updateColumnTransposeAndPrice": (ctypes.c_int, [ctypes.c_void_p, c_double_p, c_double_p]),

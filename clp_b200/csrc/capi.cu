@@ -114,9 +114,6 @@ Clpb_Simplex *Clpb_presolvedModel(Clpb_Simplex *model, int *status)
   red->e.factorizationFrequency = model->e.factorizationFrequency;
   red->e.batch = model->e.batch;
   red->e.useGraph = model->e.useGraph;
-  red->e.useRowPass = model->e.useRowPass;
-  red->e.usePriceTma = model->e.usePriceTma;
-  red->e.factorMode = model->e.factorMode;
   red->e.dualRowPivot = model->e.dualRowPivot;
   red->e.rank = model->e.rank;
   red->e.worldSize = model->e.worldSize;
@@ -216,34 +213,14 @@ int Clpb_setParameter(Clpb_Simplex *model, const char *key, double value)
     e.timing = value != 0.0;
   else if (k == "warmupIterations")
     e.warmupIterations = (int)value;
-  else if (k == "usePriceTma")
-    e.usePriceTma = value != 0.0;
   else if (k == "useGraph")
     e.useGraph = value != 0.0;
-  else if (k == "useRowPass")
-    e.useRowPass = value != 0.0;
-  else if (k == "pfiApplyVariant")
-    clpb::g_pfiApplyVariant = (int)value;
-  else if (k == "rowPassCtas")
-    clpb::g_rowPassCtas = (int)value;
-  else if (k == "priceIdx16")
-    e.priceIdx16 = value != 0.0;
-  else if (k == "gemvVariantF")
-    clpb::g_gemvVariantF = (int)value;
-  else if (k == "gemvVariantB")
-    clpb::g_gemvVariantB = (int)value;
-  else if (k == "gemvGridMul")
-    clpb::g_gemvGridMul = std::max(1, (int)value);
   else if (k == "objectiveOffset")
     e.objectiveOffset = value;
   else if (k == "scaling")
     e.scalingFlag = (int)value;
   else if (k == "perturbation")
     e.perturbation = (int)value;
-  else if (k == "refreshDualsEvery")
-    e.refreshDualsEvery = (int)value;
-  else if (k == "refreshPrimalsEvery")
-    e.refreshPrimalsEvery = (int)value;
   else if (k == "hotStart")
     e.hotStart = value != 0.0;
   else if (k == "dualRowPivot")
@@ -252,8 +229,6 @@ int Clpb_setParameter(Clpb_Simplex *model, const char *key, double value)
     e.shardPanelMode = (int)value;
   else if (k == "shardMinNnzPerRank")
     e.shardMinNnzPerRank = (long long)value;
-  else if (k == "factorMode")
-    e.factorMode = (int)value;
   else if (k == "acceptablePivot")
     e.acceptablePivot = value;
   else
@@ -549,13 +524,6 @@ int Clpb_transposeTimesPacked(Clpb_Simplex *model, double scalar, int numberPi, 
     model->e.transposeTimes(scalar, pi.data(), z.data());
     *numberZ = packDense(z, model->e.zeroTolerance, indexZ, elementZ);
     return 0;
-  });
-}
-int Clpb_dualColumnRowPass(Clpb_Simplex *model, const double *alphaRow, const double *dj,
-                           const unsigned char *status, int direction, double infeasibility, double *theta)
-{
-  return guarded([&] {
-    return model->e.dualColumnTest(alphaRow, dj, status, direction, infeasibility, theta, true);
   });
 }
 int Clpb_startup(Clpb_Simplex *model)

@@ -285,7 +285,7 @@ int Engine::setupDevice()
   // rebuilds it instead of being silently ignored
   const long long signature = (long long)scalingFlag * 1000003ll + (long long)factorizationFrequency * 101ll +
                               (timing ? 7 : 0) + (long long)worldSize * 13ll + (long long)rank * 17ll +
-                              (usePriceTma ? 3 : 0) + (long long)factorMode * 29ll + (shardActive() ? 31 : 0) + (long long)(shardPanelMode + 1) * 37ll + (long long)dualRowPivot * 41ll + (priceIdx16 ? 43 : 0);
+                              (shardActive() ? 31 : 0) + (long long)(shardPanelMode + 1) * 37ll + (long long)dualRowPivot * 41ll;
   if (deviceReady && signature == readySignature)
     return 0;
   if (deviceReady)
@@ -312,62 +312,12 @@ int Engine::setupDevice()
   p = dalloc<int>(n + 1);
   CUDA_OK(cudaMemcpy(p, hColStart.data(), sizeof(int) * (n + 1), cudaMemcpyHostToDevice));
   d.colStart = p;
-  p = dalloc<int>(nnz + 16); // padding: TMA tiles are rounded to 16-byte granules
-  CUDA_OK(cudaMemset(p, 0, sizeof(int) * (nnz + 16)));
+  p = dalloc<int>(nnz);
   CUDA_OK(cudaMemcpy(p, hRow.data(), sizeof(int) * nnz, cudaMemcpyHostToDevice));
   d.rowIdx = p;
-  d.rowIdx16 = nullptr;
-  if (m <= 65535 && priceIdx16) {
-    std::vector<unsigned short> r16((size_t)nnz + 32, 0);
-    for (long long e = 0; e < nnz; e++)
-      r16[e] = (unsigned short)hRow[e];
-    unsigned short *p16 = dalloc<unsigned short>(nnz + 32);
-    CUDA_OK(cudaMemcpy(p16, r16.data(), sizeof(unsigned short) * (nnz + 32), cudaMemcpyHostToDevice));
-    d.rowIdx16 = p16;
-  }
-  q = dalloc<double>(nnz + 16);
-  CUDA_OK(cudaMemset(q, 0, sizeof(double) * (nnz + 16)));
+  q = dalloc<double>(nnz);
   CUDA_OK(cudaMemcpy(q, wVal.data(), sizeof(double) * nnz, cudaMemcpyHostToDevice));
   d.val = q;
-  {
-    // cut this rank's column range into tiles of whole columns, <= kPriceTile entries each
-    const bool sh = shardActive();
-    int per = sh ? (n + worldSize - 1) / worldSize : n;
-    int cb = sh ? std::min(n, rank * per) : 0;
-    int ce = sh ? std::min(n, cb + per) : n;
-    std::vector<int> tiles;
-    bool ok = true;
-    int c = cb;
-    while (c < ce && ok) {
-      tiles.push_back(c);
-      const int ea = hColStart[c] & ~3;
-      int c1 = c;
-      while (c1 < ce && c1 - c < kPriceTileCols && ((hColStart[c1 + 1] + 3) & ~3) - ea <= kPriceTile)
-        c1++;
-      if (c1 == c)
-        ok = false; // a single column does not fit a tile: the LDG-direct kernel is used
-      c = c1;
-    }
-    tiles.push_back(ce);
-    d.priceTileCol = nullptr;
-    d.numPriceTiles = 0;
-    const int ntl = (int)tiles.size() - 1;
-    if (ok && ce > cb && usePriceTma) {
-      std::vector<int> desc((size_t)ntl * 4);
-      for (int t = 0; t < ntl; t++) {
-        const int t0 = tiles[t], t1 = tiles[t + 1];
-        const int ea = hColStart[t0] & ~3;
-        desc[4 * t + 0] = t0;
-        desc[4 * t + 1] = t1 - t0;
-        desc[4 * t + 2] = ea;
-        desc[4 * t + 3] = ((hColStart[t1] + 3) & ~3) - ea;
-      }
-      int *pt = dalloc<int>(desc.size());
-      CUDA_OK(cudaMemcpy(pt, desc.data(), sizeof(int) * desc.size(), cudaMemcpyHostToDevice));
-      d.priceTileCol = pt;
-      d.numPriceTiles = ntl;
-    }
-  }
   p = dalloc<int>(m + 1);
   CUDA_OK(cudaMemcpy(p, rowStart.data(), sizeof(int) * (m + 1), cudaMemcpyHostToDevice));
   d.rowStart = p;
@@ -453,18 +403,13 @@ int Engine::setupDevice()
   d.mu = dalloc<double>((size_t)3 * d.tmax);
   d.nu = dalloc<double>(d.tmax);
   d.histWeight = dalloc<unsigned long long>(kHistBuckets);
-  d.histMin = dalloc<unsigned long long>(kHistBuckets);
   d.hist2Weight = dalloc<unsigned long long>(kHist2Buckets);
   d.hist2Min = dalloc<unsigned long long>(kHist2Buckets);
   d.segTotal = dalloc<unsigned long long>(kHistBuckets / 1024);
   d.segLast = dalloc<int>(kHistBuckets / 1024);
-  d.scanCounter = dalloc<unsigned int>(1);
-  CUDA_OK(cudaMemset(d.scanCounter, 0, sizeof(unsigned int)));
   CUDA_OK(cudaMemset(d.hist2Weight, 0, sizeof(unsigned long long) * kHist2Buckets));
   CUDA_OK(cudaMemset(d.hist2Min, 0xFF, sizeof(unsigned long long) * kHist2Buckets));
   d.flipList = dalloc<int>(nm);
-  d.flipBits = dalloc<unsigned int>((nm + 31) / 32 + 4);
-  CUDA_OK(cudaMemset(d.flipBits, 0, sizeof(unsigned int) * ((nm + 31) / 32 + 4)));
   d.st = dalloc<IterState>(1);
   d.fd = dalloc<FactorDesc>(1);
   CUDA_OK(cudaMemset(d.fd, 0, sizeof(FactorDesc)));
@@ -526,7 +471,6 @@ int Engine::setupDevice()
   CUDA_OK(cudaMemset(d.fake, 0, nm));
   CUDA_OK(cudaMemset(d.dj, 0, sizeof(double) * nm));
   CUDA_OK(cudaMemset(d.histWeight, 0, sizeof(unsigned long long) * kHistBuckets));
-  CUDA_OK(cudaMemset(d.histMin, 0xFF, sizeof(unsigned long long) * kHistBuckets));
   CUDA_OK(cudaMemset(d.st, 0, sizeof(IterState)));
   if (timing) {
     events.resize(16 * 8 + 2);
@@ -952,9 +896,9 @@ int Engine::refresh()
 }
 
 // ---------------------------------------------------------------------------------------
-// One iteration = 17 kernels (18 when column-sharded).  CHUZR is not among them: the row of the
-// next iteration is chosen by the update kernel of the previous one, and launch_chuzr() runs once
-// at the start of every batch (enqueueBatchStart).
+// One iteration = 10 kernels (kernelLaunches counts 2 more when column-sharded).  CHUZR is not among
+// them: the row of the next iteration is chosen by the update kernel of the previous one, and
+// launch_chuzr() runs once at the start of every batch (enqueueBatchStart).
 void Engine::enqueueIteration(bool timed, int slot)
 {
   cudaEvent_t *ev = timed ? &events[(size_t)slot * 8] : nullptr;
@@ -964,51 +908,37 @@ void Engine::enqueueIteration(bool timed, int slot)
   launch_btran_unit(d, true, stream);
   if (timed)
     cudaEventRecord(ev[2], stream);
-  bool rowPassed = false;
   if (d.shardW > 1) {
     // column-sharded pricing: this rank's block of raw dot products, then ONE exchange per pricing
     // pass -- an in-place all-gather of the row shards (padded to 'per' entries; the padding lands
-    // on the slack part of the row, which the row kernels recompute from rho).  Everything after
+    // on the slack part of the row, which the row pass recomputes from rho).  Everything after
     // the gather runs replicated on identical data.
     int per = (n + worldSize - 1) / worldSize;
     int c0 = std::min(n, rank * per), c1 = std::min(n, c0 + per);
-    launch_price(d, c0, c1, false, stream);
+    launch_price(d, c0, c1, stream);
     if (allGatherFn(ncclComm, d.alphaRow, sizeof(double) * per, stream) != 0)
       throw std::runtime_error("clp_b200: all-gather of the row shards failed");
   } else {
-    launch_price(d, 0, n, false, stream);
+    launch_price(d, 0, n, stream);
   }
-  if (useRowPass)
-    rowPassed = true;
-  else
-    launch_price_slacks(d, 0, n, true, stream); // status mask, slack part, level-1 histogram
   if (timed)
     cudaEventRecord(ev[3], stream);
-  if (rowPassed) {
-    // row finalize, ratio test, dual update, flips and the FTRAN right-hand sides in one
-    // cooperative kernel (rowpass.cu)
-    if (!launch_row_pass(d, stream))
-      throw std::runtime_error("row pass launch failed");
-    if (timed) {
-      cudaEventRecord(ev[4], stream);
-      cudaEventRecord(ev[5], stream);
-    }
-  } else {
-    launch_chuzc(d, stream);
-    if (timed)
-      cudaEventRecord(ev[4], stream);
-    launch_dual_update_and_flips(d, d.flipBits, stream);
-    if (timed)
-      cudaEventRecord(ev[5], stream);
+  // row finalize, ratio test, dual update, flips and the FTRAN right-hand sides in one
+  // cooperative kernel (rowpass.cu)
+  if (!launch_row_pass(d, stream))
+    throw std::runtime_error("row pass launch failed");
+  if (timed) {
+    cudaEventRecord(ev[4], stream);
+    cudaEventRecord(ev[5], stream);
   }
-  launch_ftran_iteration(d, rowPassed, stream);
+  launch_ftran_iteration(d, stream);
   if (timed)
     cudaEventRecord(ev[6], stream);
   launch_pivot_updates(d, stream);
   if (timed)
     cudaEventRecord(ev[7], stream);
   g_kernelTimers = nullptr;
-  kernelLaunches += (rowPassed ? 3 + 1 + 1 + 4 + 1 : 3 + 2 + 4 + 3 + 5 + 1) + (d.shardW > 1 ? 2 : 0);
+  kernelLaunches += 3 + 1 + 1 + 4 + 1 + (d.shardW > 1 ? 2 : 0);
 }
 
 // start of a batch: stand-alone CHUZR (2 kernels)
@@ -1022,47 +952,36 @@ void Engine::buildIterationGraph()
 {
   if (iterGraph)
     return;
-  // Capture one iteration.  If the cooperative row-pass launch cannot be captured on this driver,
-  // capture again with the separate kernels; if that fails too, run without a graph.
-  for (int attempt = 0; attempt < 2 && !iterGraph; attempt++) {
-    cudaGraph_t graph = nullptr;
-    const long before = kernelLaunches;
-    bool ok = cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
-    if (ok) {
-      try {
-        enqueueIteration(false, 0);
-      } catch (const std::exception &) {
-        ok = false;
-      }
-      if (cudaStreamEndCapture(stream, &graph) != cudaSuccess || graph == nullptr)
-        ok = false;
+  // Capture one iteration; if capture or instantiation fails, run without a graph.
+  cudaGraph_t graph = nullptr;
+  const long before = kernelLaunches;
+  bool ok = cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
+  if (ok) {
+    try {
+      enqueueIteration(false, 0);
+    } catch (const std::exception &) {
+      ok = false;
     }
-    kernelLaunches = before;
-    if (ok) {
-      size_t numNodes = 0;
-      cudaGraphGetNodes(graph, nullptr, &numNodes);
-      kernelsPerIteration = (int)numNodes;
-      if (cudaGraphInstantiate(&iterGraph, graph, 0) != cudaSuccess) {
-        iterGraph = nullptr;
-        ok = false;
-      }
-    }
-    if (graph)
-      cudaGraphDestroy(graph);
-    if (!ok) {
-      cudaGetLastError(); // clear the sticky capture error
-      if (useRowPass) {
-        fprintf(stderr, "clp_b200: cooperative row pass not capturable, using the separate kernels\n");
-        useRowPass = false;
-      } else {
-        fprintf(stderr, "clp_b200: CUDA graph capture failed, launching kernels directly\n");
-        useGraph = false;
-        return;
-      }
+    if (cudaStreamEndCapture(stream, &graph) != cudaSuccess || graph == nullptr)
+      ok = false;
+  }
+  kernelLaunches = before;
+  if (ok) {
+    size_t numNodes = 0;
+    cudaGraphGetNodes(graph, nullptr, &numNodes);
+    kernelsPerIteration = (int)numNodes;
+    if (cudaGraphInstantiate(&iterGraph, graph, 0) != cudaSuccess) {
+      iterGraph = nullptr;
+      ok = false;
     }
   }
-  if (!iterGraph)
+  if (graph)
+    cudaGraphDestroy(graph);
+  if (!ok) {
+    cudaGetLastError(); // clear the sticky capture error
+    fprintf(stderr, "clp_b200: CUDA graph capture failed, launching kernels directly\n");
     useGraph = false;
+  }
 }
 
 void Engine::fetchState()
@@ -1359,16 +1278,6 @@ int Engine::dual()
               numberIterations, hState->numEtas, d.k, hState->stop, hState->infeas,
               hState->thetaDual);
     const int stop = hState->stop;
-    if (done > 0 && refreshDualsEvery > 0 && hState->stop == STOP_NONE &&
-        (numberIterations / refreshDualsEvery) != ((numberIterations - done) / refreshDualsEvery)) {
-      launch_compute_duals(d, dPi, dZ, stream, true);
-      CUDA_OK(cudaMemsetAsync(dCounters, 0, sizeof(int) * 4, stream));
-      launch_make_dual_feasible(d, currentDualBound, dCounters, stream);
-      launch_compute_primals(d, dXn, dRhs, stream, true); // the flips moved nonbasic values
-    } else if (done > 0 && refreshPrimalsEvery > 0 && hState->stop == STOP_NONE &&
-               (numberIterations / refreshPrimalsEvery) != ((numberIterations - done) / refreshPrimalsEvery)) {
-      launch_compute_primals(d, dXn, dRhs, stream, true);
-    }
     if (done > 0 && currentAcceptablePivot < acceptablePivot && hState->numEtas >= 5)
       setAcceptablePivot(acceptablePivot); // acceptablePivot_ = fabs(...) once pivots() >= 5 (:2070-2074)
     if (stop == STOP_NONE) {
@@ -1589,14 +1498,13 @@ void Engine::times(double scalar, const double *x, double *y)
 }
 
 int Engine::dualColumnTest(const double *alphaRow, const double *dj, const unsigned char *stat,
-                           int sigma, double infeas, double *theta, bool rowPass)
+                           int sigma, double infeas, double *theta)
 {
   setupDevice();
   resetStateForRun();
   CUDA_OK(cudaMemcpy(d.alphaRow, alphaRow, sizeof(double) * nm, cudaMemcpyHostToDevice));
   CUDA_OK(cudaMemcpy(d.dj, dj, sizeof(double) * nm, cudaMemcpyHostToDevice));
   CUDA_OK(cudaMemcpy(d.status, stat, nm, cudaMemcpyHostToDevice));
-  CUDA_OK(cudaMemset(d.rho, 0, sizeof(double) * m));
   IterState st;
   memset(&st, 0, sizeof(st));
   st.sigma = sigma;
@@ -1604,25 +1512,19 @@ int Engine::dualColumnTest(const double *alphaRow, const double *dj, const unsig
   st.infeas = infeas;
   CUDA_OK(cudaMemcpy(d.st, &st, sizeof(st), cudaMemcpyHostToDevice));
   CUDA_OK(cudaMemsetAsync(d.histWeight, 0, sizeof(unsigned long long) * kHistBuckets, stream));
-  CUDA_OK(cudaMemsetAsync(d.histMin, 0xFF, sizeof(unsigned long long) * kHistBuckets, stream));
   CUDA_OK(cudaMemsetAsync(d.hist2Weight, 0, sizeof(unsigned long long) * kHist2Buckets, stream));
   CUDA_OK(cudaMemsetAsync(d.hist2Min, 0xFF, sizeof(unsigned long long) * kHist2Buckets, stream));
-  if (rowPass) {
-    // the cooperative kernel of the fused iteration: it derives the slack part of the row from rho
-    // (alpha_{n+i} = -rho_i) and also runs the dual update / flips / right-hand sides that follow
-    std::vector<double> negRho(m);
-    for (int i = 0; i < m; i++)
-      negRho[i] = -alphaRow[n + i];
-    CUDA_OK(cudaMemcpy(d.rho, negRho.data(), sizeof(double) * m, cudaMemcpyHostToDevice));
-    CUDA_OK(cudaMemset(d.posToNuc, 0xFF, sizeof(int) * m)); // no factorization in this entry point
-    CUDA_OK(cudaMemsetAsync(d.segTotal, 0, sizeof(unsigned long long) * (kHistBuckets / 1024), stream));
-    CUDA_OK(cudaMemsetAsync(d.segLast, 0xFF, sizeof(int) * (kHistBuckets / 1024), stream));
-    if (!launch_row_pass(d, stream))
-      throw std::runtime_error("row pass launch failed");
-  } else {
-    launch_histogram(d, stream);
-    launch_chuzc(d, stream);
-  }
+  CUDA_OK(cudaMemsetAsync(d.segTotal, 0, sizeof(unsigned long long) * (kHistBuckets / 1024), stream));
+  CUDA_OK(cudaMemsetAsync(d.segLast, 0xFF, sizeof(int) * (kHistBuckets / 1024), stream));
+  // the row pass derives the slack part of the row from rho (alpha_{n+i} = -rho_i)
+  std::vector<double> negRho(m);
+  for (int i = 0; i < m; i++)
+    negRho[i] = -alphaRow[n + i];
+  CUDA_OK(cudaMemcpy(d.rho, negRho.data(), sizeof(double) * m, cudaMemcpyHostToDevice));
+  if (!factorsValid) // no factorization: no position is in the nucleus (the row pass reads the map)
+    CUDA_OK(cudaMemset(d.posToNuc, 0xFF, sizeof(int) * m));
+  if (!launch_row_pass(d, stream))
+    throw std::runtime_error("row pass launch failed");
   fetchState();
   *theta = hState->thetaDual;
   if (hState->stop != 0)
@@ -1683,7 +1585,7 @@ int Engine::pivotRowStep(int *sequenceOut, int *direction, double *infeasibility
 int Engine::btranPriceStep(double *rho, double *alphaRow)
 {
   launch_btran_unit(d, true, stream);
-  launch_price(d, 0, n, false, stream);
+  launch_price(d, 0, n, stream);
   kernelLaunches += 4;
   std::vector<double> r(m);
   CUDA_OK(cudaMemcpyAsync(r.data(), d.rho, sizeof(double) * m, cudaMemcpyDeviceToHost, stream));
@@ -1717,7 +1619,7 @@ int Engine::dualColumnStep(double *theta, double *alpha)
 
 double Engine::updateWeightsStep(int *returnCode)
 {
-  launch_ftran_iteration(d, true, stream);
+  launch_ftran_iteration(d, stream);
   kernelLaunches += 4;
   fetchState();
   int rc = 0;

@@ -33,12 +33,6 @@ constexpr double kDevexTryNorm = 1.0e-4; // DEVEX_TRY_NORM ClpSimplex.hpp:2056
 constexpr int kHistBuckets = 32768;       // ratio-test histogram level 1: 11 exponent + 4 mantissa bits
 constexpr int kHist2Buckets = 4096;       // level 2: the next 12 mantissa bits inside the crossing bucket
 constexpr int kMaxFlips = 8192;
-constexpr int kPriceTile = 1024;          // entries per TMA-staged tile of the CSC arrays
-constexpr int kPriceStages = 2;           // tiles in flight per pipeline
-constexpr int kPriceGroups = 4;           // independent 256-thread pipelines per CTA
-constexpr int kPriceMaxTilesPerCta = 1024; // descriptors staged in shared memory per CTA
-constexpr int kPriceTileAlloc = kPriceTile + 8;
-constexpr int kPriceTileCols = 8;         // columns per tile (one warp each)
 
 // SMs of the current device (132 on an H100 SXM), queried once: one process drives one device.
 // Grid-stride launches are sized in multiples of it.
@@ -84,8 +78,7 @@ struct IterState {
   int bucket1;           // level-1 ratio bucket in which the BFRT slope is exhausted (-1: none)
   unsigned long long residual; // fixed-point slope still to absorb inside bucket1
   // bound-flip right-hand side in fixed point (order independent => bit-identical on every rank)
-  unsigned long long flipMaxBits; // max range (u-l) over this iteration's flips (double bits)
-  double flipScale, flipInvScale; // contribution * flipScale is accumulated as int64
+  unsigned long long flipMaxBits; // max range (u-l) over this iteration's flips (double bits): sets the scale
   // acceptable pivot of the ratio test (ClpSimplexDual::acceptablePivot_): lives here and not in
   // DeviceModel because the driver relaxes it (ClpSimplexDual.cpp:2072-2074) while the captured
   // iteration graph holds DeviceModel by value
@@ -119,13 +112,10 @@ struct DeviceModel {
   // column copy (CSC) and row copy (CSR) of A
   const int *colStart;
   const int *rowIdx;
-  const unsigned short *rowIdx16; // the same row indices in 16 bits when m <= 65535 (PRICE streams these), else nullptr
   const double *val;
   const int *rowStart;
   const int *colIdx;
   const double *rval;
-  const int *priceTileCol; // [numPriceTiles] int4 descriptors {firstCol, nCols, firstEntry, nEntries}
-  int numPriceTiles;
   // rim, length n+m (columns then rows, Clp order)
   double *cost, *costTrue, *lower, *upper, *lowerTrue, *upperTrue, *sol, *dj;
   unsigned char *status, *fake;
@@ -171,13 +161,10 @@ struct DeviceModel {
   double *nu;         // [tmax]
   // ratio test
   unsigned long long *histWeight; // [kHistBuckets] fixed-point slope per ratio bucket
-  unsigned long long *histMin;    // [kHistBuckets] min ratio bits per bucket
   unsigned long long *hist2Weight, *hist2Min; // [kHist2Buckets] second level
   unsigned long long *segTotal;   // [kHistBuckets/1024] per-segment totals of the level-1 scan
   int *segLast;                   // last non-empty bucket per segment
-  unsigned int *scanCounter;      // last-block-done ticket
-  int *flipList;      // [n+m] flipped sequences of this iteration, ascending
-  unsigned int *flipBits; // [(n+m+31)/32] bit mask of the same (cleared by CHUZR)
+  int *flipList;      // [n+m] flipped sequences of this iteration (unordered)
   IterState *st;
   IterRecord *rec;    // ring of records (device)
   int recCap;
@@ -202,10 +189,6 @@ struct KernelTimers {
   cudaEvent_t price[2], ftranGemv[2], btranGemv[2];
 };
 extern KernelTimers *g_kernelTimers; // nullptr outside timing mode (engine.cu)
-extern int g_pfiApplyVariant;         // solve.cu
-extern int g_priceIdx16;              // price.cu
-extern int g_rowPassCtas;             // rowpass.cu
-extern int g_gemvVariantF, g_gemvVariantB, g_gemvGridMul; // solve.cu (launch-shape experiments)
 // collectives of a sharded run (host side; set by Engine before it enqueues work)
 struct ShardCtx {
   int W = 1, rank = 0;
@@ -218,28 +201,24 @@ extern ShardCtx g_shardCtx;           // solve.cu
 // solve.cu
 void launch_ftran(const DeviceModel &d, int nrhs, bool applyEtas, cudaStream_t s);
 void launch_btran_unit(const DeviceModel &d, bool checkState, cudaStream_t s); // rho = B^-T e_r (r = st->pivotRow)
-void launch_ftran_iteration(const DeviceModel &d, bool pregathered, cudaStream_t s); // 3 rhs + etas + pivot scalars (tail)
+void launch_ftran_iteration(const DeviceModel &d, cudaStream_t s); // 3 rhs + etas + pivot scalars (tail)
 // rowpass.cu
 bool launch_row_pass(const DeviceModel &d, cudaStream_t s);
 void launch_eta_rowvec(const DeviceModel &d, int mode, bool checkState, cudaStream_t s);
 void launch_ftran_buffer(const DeviceModel &d, double *buf, int nrhs, bool applyEtas, cudaStream_t s);
 void launch_btran_dense(const DeviceModel &d, double *vec, bool applyEtas, cudaStream_t s); // vec(m) in/out
 // price.cu
-void launch_price(const DeviceModel &d, int colBegin, int colEnd, bool fuseHistogram, cudaStream_t s);
-void launch_price_slacks(const DeviceModel &d, int colBegin, int colEnd, bool fuseHistogram, cudaStream_t s);
-void launch_histogram(const DeviceModel &d, cudaStream_t s);
+void launch_price(const DeviceModel &d, int colBegin, int colEnd, cudaStream_t s);
 void launch_transpose_times(const DeviceModel &d, const double *pi, double *z, double scalar,
                             cudaStream_t s);
 void launch_times_rows(const DeviceModel &d, const double *x, double *y, double scalar,
                        cudaStream_t s);
-void launch_chuzc(const DeviceModel &d, cudaStream_t s);
 // update.cu
 void launch_chuzr(const DeviceModel &d, cudaStream_t s); // stand-alone CHUZR (start of a batch)
-void launch_dual_update_and_flips(const DeviceModel &d, unsigned int *flipBits, cudaStream_t s);
 void launch_pivot_updates(const DeviceModel &d, cudaStream_t s);
 void launch_make_dual_feasible(const DeviceModel &d, double dualBound, int *counters, cudaStream_t s);
 void launch_compute_primals(const DeviceModel &d, double *xn, double *rhs, cudaStream_t s, bool withEtas = false);
-void launch_compute_duals(const DeviceModel &d, double *pi, double *z, cudaStream_t s, bool withEtas = false);
+void launch_compute_duals(const DeviceModel &d, double *pi, double *z, cudaStream_t s);
 void launch_objective(const DeviceModel &d, double *out, cudaStream_t s);
 void launch_primal_drift(const DeviceModel &d, const double *xold, unsigned long long *out, cudaStream_t s);
 void launch_permute_weights(const double *wOld, double *wNew, const int *srcPos, int m,

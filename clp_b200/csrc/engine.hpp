@@ -46,17 +46,8 @@ public:
   // 1 ClpDualRowDantzig (src/ClpDualRowDantzig.cpp:56 pivotRow: largest primal infeasibility)
   int dualRowPivot = 0;
   int batch = 16;                 // iterations enqueued per host synchronisation
-  int refreshDualsEvery = 0, refreshPrimalsEvery = 0; // experiments: recompute from scratch inside a cycle
   bool timing = false;
   bool useGraph = true;
-  // 16-bit row indices for PRICE (m <= 65535): 10 instead of 12 bytes per entry.  No gain at C2 -- the
-  // kernel is bound by the shared-memory gathers of rho, not by HBM -- so off
-  bool priceIdx16 = false;
-  bool usePriceTma = false;       // TMA-staged price kernel (default: LDG-direct kernel, 26% faster)
-  // 0 = choose per basis (block-banded nucleus when it pays), 1 = always the dense nucleus inverse,
-  // 2 = always block-banded (tests)
-  int factorMode = 0;
-  bool useRowPass = true;         // cooperative row-pass kernel (false / column-sharded: separate kernels)
   int warmupIterations = 0;       // device-timed window starts once this many iterations ran
   double timedMilliseconds = 0.0; // CUDA-event time of the window (iterations + refactorizations)
   int timedIterations = 0;
@@ -127,7 +118,7 @@ public:
   void transposeTimes(double scalar, const double *pi, double *z);
   void times(double scalar, const double *x, double *y);
   int dualColumnTest(const double *alphaRow, const double *dj, const unsigned char *stat,
-                     int sigma, double infeas, double *theta, bool rowPass = false);
+                     int sigma, double infeas, double *theta);
   int iterate(int count);                   // run 'count' iterations from the current state
   // ---- the iteration one plug-in call at a time (ClpDualRowPivot / ClpFactorization / ClpMatrixBase
   // methods in the order ClpSimplexDual::whileIterating calls them); device state carries over

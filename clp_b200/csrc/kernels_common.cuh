@@ -1,4 +1,4 @@
-// kernels_common.cuh -- device helpers shared by solve.cu / price.cu / update.cu.
+// kernels_common.cuh -- device helpers shared by solve.cu / price.cu / rowpass.cu / update.cu.
 #pragma once
 #include "engine.cuh"
 
@@ -15,8 +15,7 @@ __device__ __forceinline__ double warp_sum(double v)
 }
 
 // indices into DeviceModel::tailCounter
-enum : int { TAIL_DUAL_UPDATE = 0, TAIL_ITER_UPDATE = 1, TAIL_PFI_APPLY = 2, TAIL_HIST2 = 3,
-             TAIL_SELECT = 4, TAIL_SPREAD = 5 };
+enum : int { TAIL_ITER_UPDATE = 0, TAIL_PFI_APPLY = 1, TAIL_SPREAD = 2 };
 
 // "last block done": returns true in exactly one CTA of a 1-D grid, after every other CTA of the
 // grid has passed this point (and hence finished the work before it).  What the tail then reads
@@ -99,7 +98,7 @@ __device__ __forceinline__ void pivot_scalars_body(const DeviceModel &d)
   st->thetaPrimal = (valueOut - bound) / ac;
 }
 
-// ---- ratio test (CHUZC) helpers shared by price.cu and rowpass.cu
+// ---- ratio test (CHUZC) helpers of rowpass.cu
 constexpr unsigned long long kFixOne = 1ull << 40; // fixed-point 1.0 (== infeasibility)
 constexpr unsigned long long kFixCap = 1ull << 41;
 constexpr unsigned long long kSentinel = 0xFFFFFFFFFFFFFFFFull;

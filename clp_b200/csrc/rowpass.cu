@@ -1,11 +1,17 @@
 // rowpass.cu -- everything the iteration does with the tableau row, in ONE cooperative kernel.
 //
-// Replaces (single-GPU path) nine dependent launches -- row_finalize, chuzc_scan1, chuzc_hist2,
-// chuzc_harris, chuzc_select, dual_update, flip_scatter, build_rhs3, gather_nucleus -- i.e. the
-// second half of ClpPackedMatrix::transposeTimes (status mask / zero tolerance,
+// The second half of ClpPackedMatrix::transposeTimes (status mask / zero tolerance,
 // /root/reference/src/ClpPackedMatrix.cpp:1860-1900), ClpSimplexDual::dualColumn0 / dualColumn
 // (src/ClpSimplexDual.cpp:3665 / :4192), ClpSimplexDual::updateDualsInDual (:2430) with its
 // bound flips, and the unpack of the entering column (ClpPackedMatrix::unpack :4803).
+//
+// Ratio test without a sort: every candidate adds its slope contribution |alpha_j|*(u_j-l_j) to a
+// histogram over the (monotone) bit pattern of its ratio d_j/|alpha_j| -- in 2^-40 fixed point
+// relative to the primal infeasibility, with integer atomics, so the result does not depend on the
+// order of the atomics.  The bucket in which the slope of the dual objective is exhausted gives
+// theta*; the Harris bound beyond theta* and the largest |alpha| inside [theta*, harris] pick the
+// pivot.  Candidates with a ratio below theta* are "passed": the dual update flips them to their
+// other bound (BFRT).
 //
 // One CTA per SM (cooperative launch => co-resident), 1024 threads; every thread owns E entries
 // of the row and keeps (alpha, |alpha|, d~, range, flags) in registers across the phases, so the
@@ -20,9 +26,10 @@
 //   P8 flip columns -> fixed-point accumulator; entering column -> aqBuf| barrier
 //   P9 three FTRAN right-hand sides rhs3 and their nucleus gather xg
 // All reductions are order independent (integer atomics, min/max of packed keys) or done in a
-// fixed order, exactly as in the separate kernels (price.cu / update.cu), which remain the path
-// of column-sharded runs.
+// fixed order.
 #include "kernels_common.cuh"
+
+#include <cstdio>
 
 namespace clpb {
 
@@ -585,32 +592,30 @@ __global__ void __launch_bounds__(1024, 1) row_pass_kernel(DeviceModel d)
   }
 }
 
-// Launch; returns false if the row is too long for the register-resident variant (caller falls
-// back to the separate kernels).
-int g_rowPassCtas = 0;
-
+// Launch; returns false (and says why on stderr) when the row does not fit: at most 8 entries per
+// thread of one 1024-thread CTA per SM, i.e. n+m <= 8 x SMs x 1024, and at least one CTA per level-1
+// histogram segment (32 SMs).  Nothing else runs the ratio test.
 bool launch_row_pass(const DeviceModel &d, cudaStream_t s)
 {
   const int numSMs = device_sm_count();
-  // "rowPassCtas" (A/B): fewer CTAs make the grid barriers cheaper but every thread owns more entries
-  int ctas = g_rowPassCtas > 0 ? (g_rowPassCtas < numSMs ? g_rowPassCtas : numSMs) : numSMs;
-  if (ctas < kHistBuckets / 1024)
-    ctas = kHistBuckets / 1024;
-  const long gthreads = (long)ctas * 1024;
+  const long gthreads = (long)numSMs * 1024;
   const int need = (int)((d.nm + gthreads - 1) / gthreads);
-  if (need > 8 || numSMs < kHistBuckets / 1024)
+  if (need > 8 || numSMs < kHistBuckets / 1024) {
+    fprintf(stderr, "clp_b200: the row pass needs n+m <= 8 x SMs x 1024 = %ld and at least %d SMs; n+m = %d, SMs = %d\n",
+            8 * gthreads, kHistBuckets / 1024, d.nm, numSMs);
     return false;
+  }
   DeviceModel dm = d;
   void *args[] = {&dm};
   cudaError_t rc;
   if (need <= 1)
-    rc = cudaLaunchCooperativeKernel((void *)row_pass_kernel<1>, dim3(ctas), dim3(1024), args, 0, s);
+    rc = cudaLaunchCooperativeKernel((void *)row_pass_kernel<1>, dim3(numSMs), dim3(1024), args, 0, s);
   else if (need <= 2)
-    rc = cudaLaunchCooperativeKernel((void *)row_pass_kernel<2>, dim3(ctas), dim3(1024), args, 0, s);
+    rc = cudaLaunchCooperativeKernel((void *)row_pass_kernel<2>, dim3(numSMs), dim3(1024), args, 0, s);
   else if (need <= 4)
-    rc = cudaLaunchCooperativeKernel((void *)row_pass_kernel<4>, dim3(ctas), dim3(1024), args, 0, s);
+    rc = cudaLaunchCooperativeKernel((void *)row_pass_kernel<4>, dim3(numSMs), dim3(1024), args, 0, s);
   else
-    rc = cudaLaunchCooperativeKernel((void *)row_pass_kernel<8>, dim3(ctas), dim3(1024), args, 0, s);
+    rc = cudaLaunchCooperativeKernel((void *)row_pass_kernel<8>, dim3(numSMs), dim3(1024), args, 0, s);
   return rc == cudaSuccess;
 }
 

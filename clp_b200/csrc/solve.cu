@@ -22,9 +22,6 @@ namespace clpb {
 static inline int roundUp8(int v) { return (v + 7) / 8 * 8; }
 
 ShardCtx g_shardCtx;
-// launch-shape experiments (tests/ab_probe.py): rows per CTA pass / 16-byte loads in flight / CTAs per SM
-int g_gemvVariantF = 0, g_gemvVariantB = 0, g_gemvGridMul = 8;
-int g_pfiApplyVariant = 0; // 0: warp per panel row, 1: GEMV-shaped (two rows per CTA); "pfiApplyVariant"
 
 // ---------------------------------------------------------------------------------------
 // gather b_N : xg[c][j] = b_c[nucRow[j]]
@@ -136,56 +133,6 @@ __global__ void __launch_bounds__(256)
       }
     }
     __syncthreads();
-  }
-}
-
-// Same product with one WARP per row (no block-level reduction, no __syncthreads): lanes stride the row
-// in 16-byte pieces, DEPTH loads per lane in flight.  Launch-shape experiment (gemvVariantF = 7 /
-// gemvVariantB = 6); not sharded.
-template <int NRHS, int DEPTH>
-__global__ void __launch_bounds__(256)
-    gemv_warp_rows_kernel(const FactorDesc *__restrict__ fd, int transposed, const double *__restrict__ x,
-                          double *__restrict__ out, int ostride, const int *__restrict__ outIndex,
-                          const IterState *st, bool checkState)
-{
-  if (checkState && !iter_active(st))
-    return;
-  const int k = fd->k, ldk = fd->ldk;
-  const double *__restrict__ M = transposed ? fd->NinvT : fd->Ninv;
-  const int lane = threadIdx.x & 31;
-  const int half = ldk >> 1;
-  const int warpsTotal = gridDim.x * (blockDim.x >> 5);
-  for (int i = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); i < k; i += warpsTotal) {
-    const double2 *row = reinterpret_cast<const double2 *>(M + (size_t)i * ldk);
-    double acc[NRHS];
-#pragma unroll
-    for (int c = 0; c < NRHS; c++)
-      acc[c] = 0.0;
-    for (int j = lane; j < half; j += 32 * DEPTH) {
-      double2 a[DEPTH];
-#pragma unroll
-      for (int u = 0; u < DEPTH; u++)
-        a[u] = j + 32 * u < half ? __ldcs(row + j + 32 * u) : make_double2(0.0, 0.0);
-#pragma unroll
-      for (int u = 0; u < DEPTH; u++) {
-        const int jj = min(j + 32 * u, half - 1);
-#pragma unroll
-        for (int c = 0; c < NRHS; c++) {
-          const double2 xv = __ldg(reinterpret_cast<const double2 *>(x + (size_t)c * ldk) + jj);
-          acc[c] = fma(a[u].x, xv.x, acc[c]);
-          acc[c] = fma(a[u].y, xv.y, acc[c]);
-        }
-      }
-    }
-#pragma unroll
-    for (int c = 0; c < NRHS; c++) {
-      const double v = warp_sum(acc[c]);
-      if (lane == 0) {
-        const int o = outIndex ? outIndex[i] : i;
-        const int os = ostride < 0 ? ldk : ostride;
-        out[(size_t)c * os + o] = v;
-      }
-    }
   }
 }
 
@@ -322,89 +269,6 @@ __global__ void __launch_bounds__(256) pfi_mu_kernel(DeviceModel d, bool checkSt
   }
 }
 
-// x_c[p] -= sum_{i<t} W[p][i] * mu_c[i] : a GEMV over the first t columns of the m x tmax panel,
-// same shape as gemv_rows_kernel (one CTA streams R = 2 rows, DEPTH = 2 sixteen-byte loads per row in
-// flight per thread; mu goes through L1).  pivotTail: the last CTA then evaluates the accuracy gate
-// and the primal step (pivot_scalars_body) on the finished columns.
-template <int NRHS>
-__global__ void __launch_bounds__(256) pfi_apply_kernel(DeviceModel d, double *__restrict__ x, int xstride,
-                                                        bool checkState, bool pivotTail)
-{
-  constexpr int R = 2, DEPTH = 2;
-  __shared__ double part[8][R * NRHS];
-  if (checkState && !iter_active(d.st))
-    return;
-  const int t = d.st->numEtas;
-  if (t > 0) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int half = (t + 1) >> 1; // double2 per row; an odd t reads one stale entry, masked below
-    const int ngroups = (d.m + R - 1) / R;
-    for (int g = blockIdx.x; g < ngroups; g += gridDim.x) {
-      const int p0 = g * R;
-      const double2 *row[R];
-#pragma unroll
-      for (int r = 0; r < R; r++)
-        row[r] = reinterpret_cast<const double2 *>(d.W + (size_t)min(p0 + r, d.m - 1) * d.tmax);
-      double acc[R][NRHS];
-#pragma unroll
-      for (int r = 0; r < R; r++)
-#pragma unroll
-        for (int c = 0; c < NRHS; c++)
-          acc[r][c] = 0.0;
-      for (int j = threadIdx.x; j < half; j += 256 * DEPTH) {
-        double2 a[DEPTH][R];
-#pragma unroll
-        for (int u = 0; u < DEPTH; u++) {
-          const bool p = j + 256 * u < half;
-#pragma unroll
-          for (int r = 0; r < R; r++)
-            a[u][r] = p ? __ldcs(row[r] + j + 256 * u) : make_double2(0.0, 0.0);
-        }
-#pragma unroll
-        for (int u = 0; u < DEPTH; u++) {
-          const int jj = min(j + 256 * u, half - 1);
-          const bool second = 2 * jj + 1 < t;
-#pragma unroll
-          for (int c = 0; c < NRHS; c++) {
-            const double m0 = __ldg(d.mu + (size_t)c * d.tmax + 2 * jj);
-            const double m1 = second ? __ldg(d.mu + (size_t)c * d.tmax + 2 * jj + 1) : 0.0;
-#pragma unroll
-            for (int r = 0; r < R; r++) {
-              acc[r][c] = fma(a[u][r].x, m0, acc[r][c]);
-              acc[r][c] = fma(second ? a[u][r].y : 0.0, m1, acc[r][c]);
-            }
-          }
-        }
-      }
-#pragma unroll
-      for (int r = 0; r < R; r++)
-#pragma unroll
-        for (int c = 0; c < NRHS; c++) {
-          const double v = warp_sum(acc[r][c]);
-          if (lane == 0)
-            part[warp][r * NRHS + c] = v;
-        }
-      __syncthreads();
-      if (threadIdx.x < R * NRHS) {
-        double sum = 0.0;
-#pragma unroll
-        for (int w = 0; w < 8; w++)
-          sum += part[w][threadIdx.x];
-        const int r = threadIdx.x / NRHS, c = threadIdx.x % NRHS;
-        if (p0 + r < d.m)
-          x[(size_t)c * xstride + p0 + r] -= sum;
-      }
-      __syncthreads();
-    }
-  }
-  if (!pivotTail)
-    return;
-  if (!last_block_done(d.tailCounter + TAIL_PFI_APPLY))
-    return;
-  if (threadIdx.x == 0)
-    pivot_scalars_body(d);
-}
-
 // x_c[p] -= sum_{i<t} W[p][i] * mu_c[i]   (one warp per position, eight loads of the panel row in
 // flight per lane, 64 warps per SM).  pivotTail: the last CTA then evaluates the accuracy gate and
 // the primal step (pivot_scalars_body) on the finished columns.
@@ -505,48 +369,30 @@ static void shard_all_gather(void *buf, size_t bytesPerRank, cudaStream_t s)
     throw std::runtime_error("clp_b200: all-gather failed");
 }
 
+// iteration: the FTRAN of a simplex iteration, whose right-hand sides the row pass gathered at the
+// nucleus positions already (rowpass.cu), and whose last kernel evaluates the pivot scalars as its tail
 template <int NRHS>
 static void ftran_impl(const DeviceModel &d, double *b, bool applyEtas, bool checkState,
-                       cudaStream_t s, bool pivotTail = false, bool pregathered = false)
+                       cudaStream_t s, bool iteration = false)
 {
   const int m = d.m;
   // fixed launch shapes (grid-stride kernels read k from the device-side FactorDesc)
   const int maxk = d.m;
-  int gblocks = (roundUp8(maxk) + 255) / 256;
-  if (gblocks > device_sm_count())
-    gblocks = device_sm_count();
   double *xg = d.ywork + (size_t)3 * roundUp8(maxk);
-  if (!pregathered) // the row pass (rowpass.cu) writes xg together with the right-hand sides
+  if (!iteration) {
+    int gblocks = (roundUp8(maxk) + 255) / 256;
+    if (gblocks > device_sm_count())
+      gblocks = device_sm_count();
     gather_nucleus_kernel<<<gblocks, 256, 0, s>>>(d, b, m, xg, NRHS, checkState);
-  int blocks = maxk < device_sm_count() * g_gemvGridMul ? maxk : device_sm_count() * g_gemvGridMul;
+  }
+  const int blocks = maxk < device_sm_count() * 8 ? maxk : device_sm_count() * 8;
   if (g_kernelTimers && checkState)
     cudaEventRecord(g_kernelTimers->ftranGemv[0], s);
   const bool sharded = d.shardW > 1;
   double *y = sharded ? d.gatherY : d.ywork;
-#define CLPB_GEMV_F(R_, D_)                                                                                   \
-  gemv_rows_kernel<NRHS, R_, D_><<<blocks, 256, 0, s>>>(d.fd, 0, xg, y, -1, nullptr, d.st, checkState, d.shardW, \
-                                                        d.shardRank, d.shardPerK)
-  if (NRHS == 1)
-    CLPB_GEMV_F(1, 8);
-  else if (g_gemvVariantF == 1)
-    CLPB_GEMV_F(1, 4);
-  else if (g_gemvVariantF == 2)
-    CLPB_GEMV_F(1, 8);
-  else if (g_gemvVariantF == 3)
-    CLPB_GEMV_F(2, 4);
-  else if (g_gemvVariantF == 4)
-    CLPB_GEMV_F(4, 1);
-  else if (g_gemvVariantF == 5)
-    CLPB_GEMV_F(4, 2);
-  else if (g_gemvVariantF == 6)
-    CLPB_GEMV_F(1, 2);
-  else if (g_gemvVariantF == 7 && !sharded)
-    gemv_warp_rows_kernel<NRHS, 4><<<device_sm_count() * g_gemvGridMul, 256, 0, s>>>(d.fd, 0, xg, y, -1, nullptr, d.st, checkState);
-  else if (g_gemvVariantF == 8 && !sharded)
-    gemv_warp_rows_kernel<NRHS, 8><<<device_sm_count() * g_gemvGridMul, 256, 0, s>>>(d.fd, 0, xg, y, -1, nullptr, d.st, checkState);
-  else
-    CLPB_GEMV_F(2, 2);
-#undef CLPB_GEMV_F
+  constexpr int R = NRHS == 1 ? 1 : 2, DEPTH = NRHS == 1 ? 8 : 2;
+  gemv_rows_kernel<NRHS, R, DEPTH><<<blocks, 256, 0, s>>>(d.fd, 0, xg, y, -1, nullptr, d.st, checkState, d.shardW,
+                                                          d.shardRank, d.shardPerK);
   if (g_kernelTimers && checkState)
     cudaEventRecord(g_kernelTimers->ftranGemv[1], s);
   if (sharded)
@@ -560,17 +406,12 @@ static void ftran_impl(const DeviceModel &d, double *b, bool applyEtas, bool che
         pblocks = device_sm_count() * 8;
       pfi_apply_warp_kernel<NRHS><<<pblocks, 256, 0, s>>>(d, b, m, checkState, false);
       shard_all_gather(d.gatherP, sizeof(double) * NRHS * d.shardPerM, s);
-      pfi_merge_kernel<NRHS><<<(m + 255) / 256, 256, 0, s>>>(d, b, m, checkState, pivotTail);
-    } else if (g_pfiApplyVariant == 1) {
-      int pblocks = (m + 1) / 2;
-      if (pblocks > device_sm_count() * 8)
-        pblocks = device_sm_count() * 8;
-      pfi_apply_kernel<NRHS><<<pblocks, 256, 0, s>>>(d, b, m, checkState, pivotTail);
+      pfi_merge_kernel<NRHS><<<(m + 255) / 256, 256, 0, s>>>(d, b, m, checkState, iteration);
     } else {
       int pblocks = (m + 7) / 8;
       if (pblocks > device_sm_count() * 8)
         pblocks = device_sm_count() * 8;
-      pfi_apply_warp_kernel<NRHS><<<pblocks, 256, 0, s>>>(d, b, m, checkState, pivotTail);
+      pfi_apply_warp_kernel<NRHS><<<pblocks, 256, 0, s>>>(d, b, m, checkState, iteration);
     }
   }
 }
@@ -588,9 +429,9 @@ void launch_ftran(const DeviceModel &d, int nrhs, bool applyEtas, cudaStream_t s
 
 // The three FTRANs of a simplex iteration (a_q, rho -> tau, bound-flip column) with the eta panel
 // and, as the tail of the last kernel, the pivot accuracy gate / primal step length.
-void launch_ftran_iteration(const DeviceModel &d, bool pregathered, cudaStream_t s)
+void launch_ftran_iteration(const DeviceModel &d, cudaStream_t s)
 {
-  ftran_impl<3>(d, d.rhs3, true, true, s, true, pregathered);
+  ftran_impl<3>(d, d.rhs3, true, true, s, true);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -757,30 +598,12 @@ static void btran_tail(const DeviceModel &d, double *rhoOut, bool checkState, cu
 
 static void btran_gemv(const DeviceModel &d, double *rhoOut, bool checkState, cudaStream_t s)
 {
-  int blocks = d.m < device_sm_count() * g_gemvGridMul ? d.m : device_sm_count() * g_gemvGridMul;
+  const int blocks = d.m < device_sm_count() * 8 ? d.m : device_sm_count() * 8;
   if (g_kernelTimers && checkState)
     cudaEventRecord(g_kernelTimers->btranGemv[0], s);
   const bool sharded = d.shardW > 1;
-#define CLPB_GEMV_B(R_, D_)                                                                              \
-  gemv_rows_kernel<1, R_, D_><<<blocks, 256, 0, s>>>(d.fd, 1, d.swork, sharded ? d.gatherB : rhoOut, d.m, \
-                                                     d.nucRow, d.st, checkState, d.shardW, d.shardRank, d.shardPerK)
-  if (g_gemvVariantB == 1)
-    CLPB_GEMV_B(1, 4);
-  else if (g_gemvVariantB == 2)
-    CLPB_GEMV_B(2, 4);
-  else if (g_gemvVariantB == 3)
-    CLPB_GEMV_B(2, 8);
-  else if (g_gemvVariantB == 4)
-    CLPB_GEMV_B(4, 4);
-  else if (g_gemvVariantB == 5)
-    CLPB_GEMV_B(4, 2);
-  else if (g_gemvVariantB == 6 && !sharded)
-    gemv_warp_rows_kernel<1, 8><<<device_sm_count() * g_gemvGridMul, 256, 0, s>>>(d.fd, 1, d.swork, rhoOut, d.m, d.nucRow, d.st, checkState);
-  else if (g_gemvVariantB == 7 && !sharded)
-    gemv_warp_rows_kernel<1, 4><<<device_sm_count() * g_gemvGridMul, 256, 0, s>>>(d.fd, 1, d.swork, rhoOut, d.m, d.nucRow, d.st, checkState);
-  else
-    CLPB_GEMV_B(1, 8);
-#undef CLPB_GEMV_B
+  gemv_rows_kernel<1, 1, 8><<<blocks, 256, 0, s>>>(d.fd, 1, d.swork, sharded ? d.gatherB : rhoOut, d.m, d.nucRow,
+                                                   d.st, checkState, d.shardW, d.shardRank, d.shardPerK);
   if (g_kernelTimers && checkState)
     cudaEventRecord(g_kernelTimers->btranGemv[1], s);
   if (sharded) {

@@ -2,14 +2,14 @@
 //
 // Replaces, with device-resident state,
 //   ClpDualRowSteepest::pivotRow            /root/reference/src/ClpDualRowSteepest.cpp:179
-//   ClpSimplexDual::updateDualsInDual       src/ClpSimplexDual.cpp:2430   (+ flipBounds :6345)
 //   ClpDualRowSteepest::updateWeights       src/ClpDualRowSteepest.cpp:375 (recurrence :501-538)
 //   ClpDualRowSteepest::updatePrimalSolution src/ClpDualRowSteepest.cpp:630
 //   ClpSimplex::housekeeping                src/ClpSimplex.cpp:2065 (status / pivotVariable swap)
 //   ClpSimplexDual::changeBounds            src/ClpSimplexDual.cpp:3148 (fake bounds)
 //   ClpSimplex::computePrimals / computeDuals  src/ClpSimplex.cpp:914 / :1164
 // All reductions are order independent (packed-key atomicMax/Min, integer atomics) or done
-// in a fixed order, so replicated ranks of a column-sharded run stay bit-identical.
+// in a fixed order, so replicated ranks of a column-sharded run stay bit-identical.  The dual
+// update and the bound flips run in the row pass (rowpass.cu).
 #include "kernels_common.cuh"
 
 namespace clpb {
@@ -32,8 +32,6 @@ __global__ void chuzr_kernel(DeviceModel d)
       d.hist2Min[b] = 0xFFFFFFFFFFFFFFFFull;
     }
   }
-  for (int w = blockIdx.x * blockDim.x + threadIdx.x; w < ((d.nm + 31) >> 5); w += gridDim.x * blockDim.x)
-    d.flipBits[w] = 0u;
   if (blockIdx.x == 0 && threadIdx.x < kHistBuckets / 1024) {
     d.segTotal[threadIdx.x] = 0ull;
     d.segLast[threadIdx.x] = -1;
@@ -100,223 +98,7 @@ void launch_chuzr(const DeviceModel &d, cudaStream_t s)
   chuzr_finish_kernel<<<1, 1, 0, s>>>(d);
 }
 
-// ------------------------------------------------------------------ dual update + flips
-// Tail of dual_update_kernel (last CTA, 256 threads): ordered expansion of the flip bit mask into
-// flipList, numFlips, and the fixed-point scale of the bound-flip right-hand side.
-__device__ __forceinline__ void flip_collect_tail(const DeviceModel &d, const unsigned int *flipBits)
-{
-  __shared__ int warpCount[8];
-  __shared__ int base;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int nwords = (d.nm + 31) >> 5;
-  if (tid == 0)
-    base = 0;
-  __syncthreads();
-  for (int start = 0; start < nwords; start += 256 * 4) {
-    unsigned int w[4];
-    int cnt = 0;
-#pragma unroll
-    for (int q = 0; q < 4; q++) {
-      const int wi = start + tid * 4 + q;
-      w[q] = wi < nwords ? __ldcg(flipBits + wi) : 0u;
-      cnt += __popc(w[q]);
-    }
-    int inc = cnt;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      int t = __shfl_up_sync(0xffffffffu, inc, o);
-      if (lane >= o)
-        inc += t;
-    }
-    if (lane == 31)
-      warpCount[warp] = inc;
-    __syncthreads();
-    int off = base + inc - cnt;
-    for (int q = 0; q < warp; q++)
-      off += warpCount[q];
-#pragma unroll
-    for (int q = 0; q < 4; q++) {
-      unsigned int bits = w[q];
-      const int j0 = (start + tid * 4 + q) << 5;
-      while (bits) {
-        const int b = __ffs(bits) - 1;
-        bits &= bits - 1;
-        d.flipList[off++] = j0 + b;
-      }
-    }
-    __syncthreads();
-    if (tid == 255) {
-      int tot = 0;
-      for (int q = 0; q < 8; q++)
-        tot += warpCount[q];
-      base += tot;
-    }
-    __syncthreads();
-  }
-  if (tid == 0) {
-    IterState *st = d.st;
-    const int nf = base;
-    st->numFlips = nf;
-    if (nf > 0) {
-      // every contribution |a_ij * delta_j| <= amax * maxRange < 2^E; nf < 2^bitsN of them per row at
-      // most: with Q = 62 - bitsN fractional bits the int64 sums cannot overflow
-      const unsigned long long mb = atomicMax(&st->flipMaxBits, 0ull);
-      const double bound = d.amax * __longlong_as_double((long long)mb);
-      int E = 0;
-      frexp(bound, &E);
-      const int bitsN = 32 - __clz(nf);
-      const int Q = 62 - bitsN;
-      st->flipScale = ldexp(1.0, Q - E);
-      st->flipInvScale = ldexp(1.0, E - Q);
-    }
-    st->flipMaxBits = 0ull;
-  }
-}
-
-// dj -= thetaDual * sigma * alpha over the pivot row; variables whose dj changes sign flip to
-// the other bound when boxed, otherwise their cost is shifted (ClpSimplexDual.cpp:4705-4772).
-// flipBits marks flipped variables; the last CTA expands it into the ordered flipList.
-__global__ void __launch_bounds__(256) dual_update_kernel(DeviceModel d, unsigned int *__restrict__ flipBits)
-{
-  if (!iter_active(d.st))
-    return;
-  const double theta = d.st->thetaDual;
-  const int sigma = d.st->sigma;
-  const int seqIn = d.st->seqIn;
-  const double tol = d.dualTolerance;
-  unsigned long long maxRange = 0ull;
-  for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < d.nm; j += gridDim.x * blockDim.x) {
-    const double alpha = d.alphaRow[j];
-    if (alpha != 0.0 && j != seqIn) {
-      const unsigned char st = d.status[j];
-      if (st != basic && st != isFixed) {
-        double dnew = d.dj[j] - theta * (sigma * alpha);
-        bool wrong = (st == atLowerBound && dnew < -tol) || (st == atUpperBound && dnew > tol);
-        if (wrong) {
-          const double lo = d.lower[j], up = d.upper[j];
-          if (up - lo < 1.0e29) {
-            if (st == atLowerBound) {
-              d.status[j] = atUpperBound;
-              d.sol[j] = up;
-            } else {
-              d.status[j] = atLowerBound;
-              d.sol[j] = lo;
-            }
-            atomicOr(flipBits + (j >> 5), 1u << (j & 31));
-            maxRange = max(maxRange, (unsigned long long)__double_as_longlong(up - lo));
-          } else {
-            d.cost[j] -= dnew;
-            dnew = 0.0;
-            atomicAdd(&d.st->costShifts, 1);
-          }
-        } else if ((st == isFree || st == superBasic) && fabs(dnew) > tol) {
-          d.cost[j] -= dnew;
-          dnew = 0.0;
-          atomicAdd(&d.st->costShifts, 1);
-        }
-        d.dj[j] = dnew;
-      }
-    }
-  }
-  if (maxRange != 0ull)
-    atomicMax(&d.st->flipMaxBits, maxRange);
-  if (!last_block_done(d.tailCounter + TAIL_DUAL_UPDATE))
-    return;
-  flip_collect_tail(d, flipBits);
-}
-
-// flipAcc[i] += fixed-point( -a_ij * delta_j ) for every flipped variable j (one warp per flip;
-// the slack of row i contributes +delta).  Integer atomics: the sums do not depend on the order.
-// Replaces the reference's sparse "matrix_->add" of the flipped columns
-// (ClpSimplexDual::updateDualsInDual, src/ClpSimplexDual.cpp:2430 -> ClpPackedMatrix::add :4874).
-__global__ void __launch_bounds__(256) flip_scatter_kernel(DeviceModel d)
-{
-  if (!iter_active(d.st))
-    return;
-  const int nf = d.st->numFlips;
-  if (nf == 0)
-    return;
-  const double scale = d.st->flipScale;
-  const int lane = threadIdx.x & 31;
-  const int warpsPerBlock = blockDim.x >> 5;
-  unsigned long long *acc = reinterpret_cast<unsigned long long *>(d.flipAcc);
-  for (int f = blockIdx.x * warpsPerBlock + (threadIdx.x >> 5); f < nf; f += gridDim.x * warpsPerBlock) {
-    const int j = d.flipList[f];
-    const double range = d.upper[j] - d.lower[j];
-    const double delta = d.status[j] == atUpperBound ? range : -range;
-    if (j >= d.n) {
-      if (lane == 0)
-        atomicAdd(acc + (j - d.n), (unsigned long long)__double2ll_rn(delta * scale));
-    } else {
-      const int e1 = d.colStart[j + 1];
-      for (int e = d.colStart[j] + lane; e < e1; e += 32)
-        atomicAdd(acc + d.rowIdx[e], (unsigned long long)__double2ll_rn(-delta * d.val[e] * scale));
-    }
-  }
-}
-
-// rhs3[0] = a_q (entering column of [A|-I]); rhs3[1] = rho; rhs3[2] = bound-flip right-hand side
-// (fixed point -> double; the accumulator is left zero for the next iteration).
-__global__ void __launch_bounds__(256) build_rhs3_kernel(DeviceModel d)
-{
-  if (!iter_active(d.st))
-    return;
-  __shared__ int sRow[256];
-  __shared__ double sVal[256];
-  const int row = blockIdx.x * blockDim.x + threadIdx.x;
-  const bool live = row < d.m;
-  const int q = d.st->seqIn;
-  double aq = 0.0, fl = 0.0;
-  // entering column
-  if (q >= d.n) {
-    if (live && row == q - d.n)
-      aq = -1.0;
-  } else {
-    const int e0 = d.colStart[q], e1 = d.colStart[q + 1];
-    for (int c0 = e0; c0 < e1; c0 += 256) {
-      int e = c0 + threadIdx.x;
-      sRow[threadIdx.x] = e < e1 ? d.rowIdx[e] : -1;
-      sVal[threadIdx.x] = e < e1 ? d.val[e] : 0.0;
-      __syncthreads();
-      int cnt = min(256, e1 - c0);
-      for (int t = 0; t < cnt; t++)
-        if (sRow[t] == row)
-          aq = sVal[t];
-      __syncthreads();
-    }
-  }
-  if (live) {
-    if (d.st->numFlips > 0) {
-      const long long a = d.flipAcc[row];
-      if (a != 0ll) {
-        fl = (double)a * d.st->flipInvScale;
-        d.flipAcc[row] = 0ll;
-      }
-    }
-    d.rhs3[row] = aq;
-    d.rhs3[(size_t)d.m + row] = d.rho[row];
-    d.rhs3[(size_t)2 * d.m + row] = fl;
-  }
-}
-
-void launch_dual_update_and_flips(const DeviceModel &d, unsigned int *flipBits, cudaStream_t s)
-{
-  int blocks = (d.nm + 255) / 256;
-  if (blocks > device_sm_count() * 8)
-    blocks = device_sm_count() * 8;
-  dual_update_kernel<<<blocks, 256, 0, s>>>(d, flipBits);
-  flip_scatter_kernel<<<device_sm_count(), 256, 0, s>>>(d);
-  build_rhs3_kernel<<<(d.m + 255) / 256, 256, 0, s>>>(d);
-}
-
 // ------------------------------------------------------------------ after the FTRANs
-__global__ void pivot_scalars_kernel(DeviceModel d)
-{
-  if (!iter_active(d.st))
-    return;
-  pivot_scalars_body(d);
-}
-
 // status / pivotVariable swap and per-iteration record (ClpSimplex::housekeeping), single thread
 __device__ __forceinline__ void pivot_fixup_body(const DeviceModel &d)
 {
@@ -357,8 +139,8 @@ __device__ __forceinline__ void pivot_fixup_body(const DeviceModel &d)
 // End of an iteration in one kernel:
 //   CTAs [0, etaBlocks)      : new row of Ginv / column of GinvT from the BTRAN's nu (eta_append_row)
 //   CTAs [etaBlocks, grid)   : x_B, DSE weights (ClpDualRowSteepest.cpp:501-538) and the new eta
-//                              column, one thread per position; clear the ratio-test histograms and
-//                              the flip mask; score every position for the NEXT iteration's CHUZR
+//                              column, one thread per position; clear the ratio-test histograms;
+//                              score every position for the NEXT iteration's CHUZR
 //   tail (last CTA, thread 0): housekeeping of this iteration, then decode the next pivot row.
 __global__ void __launch_bounds__(256) iteration_update_kernel(DeviceModel d, int etaBlocks)
 {
@@ -381,8 +163,6 @@ __global__ void __launch_bounds__(256) iteration_update_kernel(DeviceModel d, in
         d.hist2Min[b] = 0xFFFFFFFFFFFFFFFFull;
       }
     }
-    for (int w = gtid; w < ((d.nm + 31) >> 5); w += gthreads)
-      d.flipBits[w] = 0u;
     if (gtid < kHistBuckets / 1024) {
       d.segTotal[gtid] = 0ull;
       d.segLast[gtid] = -1;
@@ -749,10 +529,11 @@ void launch_compute_primals(const DeviceModel &d, double *xn, double *rhs, cudaS
   launch_ftran_buffer(d, rhs, 1, withEtas, s);
   add_basic_kernel<<<(d.m + 255) / 256, 256, 0, s>>>(d, rhs);
 }
-void launch_compute_duals(const DeviceModel &d, double *pi, double *z, cudaStream_t s, bool withEtas)
+void launch_compute_duals(const DeviceModel &d, double *pi, double *z, cudaStream_t s)
 {
+  // right after a refactorization: no etas
   gather_basic_cost_kernel<<<(d.m + 255) / 256, 256, 0, s>>>(d, pi);
-  launch_btran_dense(d, pi, withEtas, s);
+  launch_btran_dense(d, pi, false, s);
   launch_transpose_times(d, pi, z, 1.0, s);
   reduced_cost_kernel<<<(d.nm + 255) / 256, 256, 0, s>>>(d, z, pi);
 }

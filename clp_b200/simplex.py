@@ -302,15 +302,6 @@ class ClpSimplex:
                                               float(infeasibility), ctypes.byref(theta)))
         return q, theta.value
 
-    def dualColumnRowPass(self, alphaRow, dj, status, direction, infeasibility):
-        a = np.ascontiguousarray(alphaRow, dtype=np.float64)
-        d = np.ascontiguousarray(dj, dtype=np.float64)
-        s = np.ascontiguousarray(status, dtype=np.uint8)
-        theta = ctypes.c_double(0.0)
-        q = self._chk(self._L.Clpb_dualColumnRowPass(self._h, _dp(a), _dp(d), _up(s), int(direction),
-                                                     float(infeasibility), ctypes.byref(theta)))
-        return q, theta.value
-
     # ---- ClpDualRowPivot surface, one iteration at a time (include/clp_b200.h)
     def pivotRow(self):
         """ClpDualRowPivot::pivotRow -> (row or -1/-2, sequenceOut, direction, infeasibility)"""

@@ -105,7 +105,10 @@ int Clpb_lastSolveWasHot(Clpb_Simplex *model);
 int Clpb_refactorizationInterval(Clpb_Simplex *model, int nucleusSize);
 /* Clp_dual :346 (ClpSimplex::dual src/ClpSimplex.cpp:5631).  Returns Clp_status :212:
    0 optimal, 1 primal infeasible, 2 dual infeasible, 3 stopped on iterations/time,
-   4 stopped due to errors. */
+   4 stopped due to errors.  The ratio test runs in one cooperative kernel whose threads hold at most
+   8 entries of the tableau row each: n+m must not exceed 8 x SMs x 1024 (1 081 344 on a 132-SM
+   H100 SXM, 933 888 on a 114-SM H100 PCIe), and the device needs at least 32 SMs.  Otherwise
+   Clpb_dual returns -99 and prints the reason on stderr. */
 int Clpb_dual(Clpb_Simplex *model, int ifValuesPass);
 int Clpb_status(Clpb_Simplex *model);
 /* Clp_objectiveValue :256, Clp_numberIterations :195 */
@@ -171,15 +174,12 @@ int Clpb_transposeTimes(Clpb_Simplex *model, double scalar, const double *pi, do
 int Clpb_times(Clpb_Simplex *model, double scalar, const double *x, double *y);
 /* ClpSimplexDual::dualColumn (src/ClpSimplexDual.cpp:4192) on an explicit tableau row:
    alphaRow[n+m], dj[n+m], status[n+m]; direction +1 leaving to upper / -1 to lower.
-   Returns sequenceIn or -1; *theta = dual step. */
+   Returns sequenceIn or -1; *theta = dual step.  Run by the cooperative row kernel of the fused
+   iteration (rowpass.cu), which also performs the dual update and the bound flips that follow it
+   on the device copy of dj / status. */
 int Clpb_dualColumn(Clpb_Simplex *model, const double *alphaRow, const double *dj,
                     const unsigned char *status, int direction, double infeasibility,
                     double *theta);
-/* The same test run by the cooperative row kernel of the fused iteration (rowpass.cu), which also
-   performs the dual update and the bound flips that follow it on the device copy of dj / status. */
-int Clpb_dualColumnRowPass(Clpb_Simplex *model, const double *alphaRow, const double *dj,
-                           const unsigned char *status, int direction, double infeasibility,
-                           double *theta);
 /* The dense kernel of the refactorization on its own (CoinAbcDgetrf + inverse,
    src/AbcSimplexParallel.cpp:2491): a[k*k] column-major in, x = a^-1 column-major out.
    Returns 0, or 1 + the index of the first column without an acceptable pivot. */

@@ -14,7 +14,6 @@ if status is not None:
     s.copyinStatus(status)
 s.setParameter("useGraph", 0); s.setParameter("batch", 8)
 s.setMaximumIterations(iters); s.setFactorizationFrequency(default_cycle(lp.m))
-if len(sys.argv) > 3: s.setParameter('usePriceTma', int(sys.argv[3]))
-if len(sys.argv) > 4: s.setLogLevel(int(sys.argv[4]))
+if len(sys.argv) > 3: s.setLogLevel(int(sys.argv[3]))
 st = s.dual()
 print("status", st, "iterations", s.numberIterations(), "nucleus", s.nucleusSize(), "objective", s.objectiveValue())

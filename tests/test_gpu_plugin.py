@@ -99,11 +99,11 @@ def _row_case(rng, nm, kind):
 
 @pytest.mark.parametrize("kind", ["plain", "ties", "boxed-small", "free", "wide"])
 @pytest.mark.parametrize("n", [20000, 400000])   # 1 and 4 entries per thread of the cooperative kernel
-def test_row_pass_kernel_against_reference_rule(kind, n):
-    """the cooperative row_pass_kernel (the kernel of the fused iteration; test_dual_column_against_oracle
-    goes through the separate fallback kernels) on adversarial rows, against the oracle's restatement of
-    the reference's SORTED-PASS dualColumn (ClpSimplexDual.cpp:4331-4658): never beyond its break point
-    and within the histogram resolution + Harris slack of it; and identical to the bucketed restatement."""
+def test_dual_column_on_adversarial_rows_against_reference_rule(kind, n):
+    """Clpb_dualColumn, i.e. the cooperative row_pass_kernel of the fused iteration, on adversarial rows, against
+    the oracle's restatement of the reference's SORTED-PASS dualColumn (ClpSimplexDual.cpp:4331-4658):
+    never beyond its break point and within the histogram resolution + Harris slack of it; and identical
+    to the bucketed restatement."""
     import zlib
 
     rng = np.random.default_rng(zlib.crc32(f"{kind}-{n}".encode()))
@@ -119,7 +119,7 @@ def test_row_pass_kernel_against_reference_rule(kind, n):
               np.zeros(n), np.zeros(m), ub[n:].copy())
     s = engine(lp)
     infeas, sigma = 3.0, 1
-    q, theta = s.dualColumnRowPass(alpha, dj, stat, sigma, infeas)
+    q, theta = s.dualColumn(alpha, dj, stat, sigma, infeas)
     idx = np.nonzero((alpha != 0) & (np.abs(alpha) > 1e-12))[0]
     rng_arg = np.where(stat == 0, 1e30, rangeb)
     args = (sigma * alpha[idx], dj[idx], rng_arg[idx], stat[idx], infeas)
