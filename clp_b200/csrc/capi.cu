@@ -336,26 +336,32 @@ int Clpb_denseInvert(int k, const double *a, double *x)
     int devCount = 0;
     if (cudaGetDeviceCount(&devCount) != cudaSuccess || devCount == 0)
       throw std::runtime_error("no CUDA device");
+    if (k <= 0)
+      return 0;
     const int ld = (k + 7) / 8 * 8;
+    const size_t bytes = sizeof(double) * (size_t)k * ld;
     double *dA = nullptr, *dX = nullptr;
-    int *dI = nullptr, *dP = nullptr, *dInfo = nullptr;
-    cudaMalloc(&dA, sizeof(double) * (size_t)k * ld);
-    cudaMalloc(&dX, sizeof(double) * (size_t)k * ld);
-    cudaMalloc(&dI, sizeof(int) * k);
-    cudaMalloc(&dP, sizeof(int) * k);
-    cudaMalloc(&dInfo, sizeof(int));
-    cudaMemset(dA, 0, sizeof(double) * (size_t)k * ld);
-    // column-major with leading dimension ld
-    cudaMemcpy2D(dA, sizeof(double) * ld, a, sizeof(double) * k, sizeof(double) * k, k, cudaMemcpyHostToDevice);
-    std::vector<int> hi(k), hp(k);
-    cudaStream_t s;
-    cudaStreamCreate(&s);
-    int info = clpb::dense_invert(dA, dX, k, ld, dI, dP, dInfo, hi.data(), hp.data(), 1.0e-11, s);
-    cudaStreamSynchronize(s);
-    if (info == 0)
-      cudaMemcpy2D(x, sizeof(double) * k, dX, sizeof(double) * ld, sizeof(double) * k, k, cudaMemcpyDeviceToHost);
-    cudaStreamDestroy(s);
-    cudaFree(dA); cudaFree(dX); cudaFree(dI); cudaFree(dP); cudaFree(dInfo);
+    cudaStream_t s = nullptr;
+    clpb::LuWorkspace w;
+    // nothing between the allocations and the releases throws: every path frees everything
+    int info = -99;
+    if (cudaMalloc(&dA, bytes) == cudaSuccess && cudaMalloc(&dX, bytes) == cudaSuccess &&
+        clpb::lu_workspace_reserve(w, k, k) == cudaSuccess && cudaStreamCreate(&s) == cudaSuccess &&
+        cudaMemset(dA, 0, bytes) == cudaSuccess &&
+        // column-major with leading dimension ld
+        cudaMemcpy2D(dA, sizeof(double) * ld, a, sizeof(double) * k, sizeof(double) * k, k,
+                     cudaMemcpyHostToDevice) == cudaSuccess) {
+      info = clpb::dense_invert(dA, dX, k, ld, w, 1.0e-11, s);
+      if (info == 0 && (cudaStreamSynchronize(s) != cudaSuccess ||
+                        cudaMemcpy2D(x, sizeof(double) * k, dX, sizeof(double) * ld, sizeof(double) * k, k,
+                                     cudaMemcpyDeviceToHost) != cudaSuccess))
+        info = -99;
+    }
+    if (s)
+      cudaStreamDestroy(s);
+    clpb::lu_workspace_release(w);
+    cudaFree(dA);
+    cudaFree(dX);
     return info;
   });
 }

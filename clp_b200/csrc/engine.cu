@@ -45,6 +45,7 @@ void Engine::freeAll()
   for (void *p : allocs)
     cudaFree(p);
   allocs.clear();
+  lu_workspace_release(lu);
   for (cudaEvent_t e : events)
     cudaEventDestroy(e);
   events.clear();
@@ -421,9 +422,7 @@ int Engine::setupDevice()
   dZ = dalloc<double>(n);
   dObj = dalloc<double>(2);
   dCounters = dalloc<int>(4);
-  dIpiv = dalloc<int>(m);
-  dPerm = dalloc<int>(m);
-  dInfo = dalloc<int>(1);
+  CUDA_OK(lu_workspace_reserve(lu, m, 0));
   CUDA_OK(cudaMallocHost(&hState, sizeof(IterState)));
   CUDA_OK(cudaMallocHost(&hRec, sizeof(IterRecord) * d.recCap));
   d.k = 0;
@@ -581,7 +580,6 @@ int Engine::refactor()
   CUDA_OK(cudaMemcpyAsync(hPivot.data(), d.pivotVariable, sizeof(int) * m, cudaMemcpyDeviceToHost,
                           stream));
   CUDA_OK(cudaStreamSynchronize(stream));
-  std::vector<int> hostIpiv(m), hostPerm(m);
   for (int attempt = 0; attempt < 200; attempt++) {
     // ---- canonical positions: basic slack of row i at position i, structurals elsewhere
     std::vector<int> newPivot(m, -1), srcPos(m, -1);
@@ -628,6 +626,7 @@ int Engine::refactor()
     if ((size_t)k * ldk > nucCap) {
       int kc = std::min(m, std::max(k + k / 4 + 64, 256));
       int ldc = roundUp(kc, 8);
+      CUDA_OK(lu_workspace_reserve(lu, m, kc));
       nucCap = (size_t)kc * ldc;
       // the old (smaller) pair is released first: at m = 5e4 a factor pair is up to 40 GB
       for (double *old : {d.Ninv, d.NinvT})
@@ -690,12 +689,11 @@ int Engine::refactor()
       struct Ctx {
         decltype(buildS1) *fn;
       } ctx{&buildS1};
-      info = dense_invert(d.NinvT, d.Ninv, k, ldk, dIpiv, dPerm, dInfo, hostIpiv.data(),
-                          hostPerm.data(), 1.0e-11, stream, d.shardW, d.shardRank,
+      info = dense_invert(d.NinvT, d.Ninv, k, ldk, lu, 1.0e-11, stream, d.shardW, d.shardRank,
                           d.shardW > 1 ? allGatherFn : nullptr, ncclComm,
                           [](void *c) { (*static_cast<Ctx *>(c)->fn)(); }, &ctx);
       if (info < 0)
-        throw std::runtime_error("clp_b200: refactorization failed (allocation or collective)");
+        throw std::runtime_error("clp_b200: refactorization failed (CUDA error or collective)");
       kernelLaunches += 6 * ((k + 31) / 32) * 2;
     } else {
       buildS1();
@@ -762,14 +760,7 @@ int Engine::refactor()
     // position whose row is dependent); bring its slack in and drop the structural that the
     // permutation had parked there (ClpFactorization.cpp:2382-2532 does the same repair).
     const int jbad = info - 1;
-    for (int i = 0; i < k; i++)
-      hostPerm[i] = i;
-    for (int j = 0; j < jbad; j++) {
-      int pp = hostIpiv[j];
-      if (pp != j)
-        std::swap(hostPerm[j], hostPerm[pp]);
-    }
-    const int seqLeave = nucCol[hostPerm[jbad]];
+    const int seqLeave = nucCol[lu.hostPerm[jbad]];
     const int rowEnter = nucRow[jbad];
     if (logLevel > 0)
       fprintf(stderr, "clp_b200: singular basis: structural %d out, slack of row %d in\n",

@@ -31,6 +31,7 @@ constexpr int NB = 32;
 // CTA knows the pivot row, the two owners exchange the rows, and all CTAs eliminate.
 constexpr int kSlabPitch = NB + 1;       // padded row pitch in shared memory (bank conflicts)
 constexpr int kPanelMaxRowsPerCta = 640; // 640 rows x 33 x 8 B = 165 KB of shared memory
+constexpr int kPanelMinRowsPerCta = 32;  // fewer, fatter CTAs make the per-column grid barrier cheaper
 
 // Monotone arrival counter (never reset inside a factorization: 'target' grows by gridDim.x per
 // barrier).  One acq_rel atomic per CTA + an acquire spin -- the formulation rowpass.cu found about
@@ -288,96 +289,6 @@ __global__ void __launch_bounds__(256)
       A[(size_t)(j0 + c) * ld + r0 + q] = slab[q * kSlabPitch + c];
 }
 
-// ---- single-CTA fallback (very tall panels that do not fit the cooperative kernel's slabs)
-__global__ void __launch_bounds__(1024)
-    lu_panel_kernel(double *__restrict__ A, int k, int ld, int j0, int nb, int *__restrict__ ipiv,
-                    int *__restrict__ info, double singularTol)
-{
-  __shared__ double sVal[32];
-  __shared__ int sIdx[32];
-  __shared__ double urow[NB];
-  __shared__ int sPiv;
-  __shared__ double sPivVal;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  for (int jj = 0; jj < nb; jj++) {
-    const int j = j0 + jj;
-    double *colj = A + (size_t)j * ld;
-    // pivot search
-    double best = -1.0;
-    int bi = j;
-    for (int i = j + tid; i < k; i += 1024) {
-      double a = fabs(colj[i]);
-      if (a > best) {
-        best = a;
-        bi = i;
-      }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      double ob = __shfl_xor_sync(0xffffffffu, best, o);
-      int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-      if (ob > best || (ob == best && oi < bi)) {
-        best = ob;
-        bi = oi;
-      }
-    }
-    if (lane == 0) {
-      sVal[warp] = best;
-      sIdx[warp] = bi;
-    }
-    __syncthreads();
-    if (warp == 0) {
-      best = sVal[lane];
-      bi = sIdx[lane];
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        double ob = __shfl_xor_sync(0xffffffffu, best, o);
-        int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-        if (ob > best || (ob == best && oi < bi)) {
-          best = ob;
-          bi = oi;
-        }
-      }
-      if (lane == 0) {
-        sPiv = bi;
-        sPivVal = best;
-        ipiv[j] = bi;
-      }
-    }
-    __syncthreads();
-    const int piv = sPiv;
-    const bool singular = !(sPivVal >= singularTol);
-    if (singular) {
-      if (tid == 0 && *info == 0)
-        *info = j + 1;
-      __syncthreads();
-      continue; // leave the column untouched; the caller repairs the basis
-    }
-    // swap rows j and piv inside the panel, cache row j of U
-    if (tid < nb) {
-      double *c = A + (size_t)(j0 + tid) * ld;
-      double a = c[j], b = c[piv];
-      if (piv != j) {
-        c[j] = b;
-        c[piv] = a;
-        a = b;
-      }
-      urow[tid] = a; // row j of the panel after the swap
-    }
-    __syncthreads();
-    const double inv = 1.0 / urow[jj];
-    for (int i = j + 1 + tid; i < k; i += 1024) {
-      double l = colj[i] * inv;
-      colj[i] = l;
-      for (int c = jj + 1; c < nb; c++) {
-        double *cc = A + (size_t)(j0 + c) * ld;
-        cc[i] = fma(-l, urow[c], cc[i]);
-      }
-    }
-    __syncthreads();
-  }
-}
-
 // Row interchanges of a panel applied to the columns left and right of it.  The nb interchanges touch
 // at most 2*nb rows; lu_perm_kernel composes them into ONE permutation of those rows (perm[0] = count,
 // perm[1+i] = touched row, perm[1+2*NB+i] = the row its final content comes from).  The elements are
@@ -569,8 +480,6 @@ bool blas_ready()
   if (g_blasState != 0)
     return g_blasState > 0;
   g_blasState = -1;
-  if (getenv("CLPB_NO_CUBLAS"))
-    return false;
   const char *names[] = {"libcublas.so.12", "/usr/local/cuda/lib64/libcublas.so.12", "libcublas.so", nullptr};
   void *h = nullptr;
   for (int i = 0; names[i] && !h; i++)
@@ -651,88 +560,109 @@ __global__ void zero_padding_kernel(double *__restrict__ M, int k, int ld)
     M[(size_t)i * ld + j] = 0.0;
 }
 
+cudaError_t lu_workspace_reserve(LuWorkspace &w, int maxK, int swapK)
+{
+  cudaError_t e = cudaSuccess;
+  auto dev = [&e](auto *&p, size_t count) {
+    if (e == cudaSuccess)
+      e = cudaMalloc(&p, sizeof(*p) * count);
+  };
+  if (!w.pubKey) {
+    const size_t sms = device_sm_count();
+    dev(w.pubKey, NB * sms);
+    dev(w.pubRows, NB * sms * NB);
+    dev(w.pubDiag, NB * NB);
+    dev(w.barrierCounter, 1);
+    dev(w.panelPerm, 1 + 4 * NB);
+    dev(w.dInfo, 1);
+  }
+  if (maxK > w.maxK) {
+    cudaFree(w.dIpiv);
+    cudaFree(w.dPerm);
+    free(w.hostIpiv);
+    free(w.hostPerm);
+    w.dIpiv = w.dPerm = w.hostIpiv = w.hostPerm = nullptr;
+    dev(w.dIpiv, maxK);
+    dev(w.dPerm, maxK);
+    w.hostIpiv = (int *)malloc(sizeof(int) * maxK);
+    w.hostPerm = (int *)malloc(sizeof(int) * maxK);
+    if (e == cudaSuccess && (!w.hostIpiv || !w.hostPerm))
+      e = cudaErrorMemoryAllocation;
+    w.maxK = maxK;
+  }
+  if (swapK > w.swapK) {
+    cudaFree(w.swapTmp);
+    w.swapTmp = nullptr;
+    dev(w.swapTmp, (size_t)2 * NB * swapK);
+    w.swapK = swapK;
+  }
+  if (e != cudaSuccess)
+    lu_workspace_release(w);
+  return e;
+}
+
+void lu_workspace_release(LuWorkspace &w)
+{
+  for (void *p : {(void *)w.dIpiv, (void *)w.dPerm, (void *)w.dInfo, (void *)w.pubKey, (void *)w.pubRows,
+                  (void *)w.pubDiag, (void *)w.barrierCounter, (void *)w.panelPerm, (void *)w.swapTmp})
+    cudaFree(p);
+  free(w.hostIpiv);
+  free(w.hostPerm);
+  w = LuWorkspace{};
+}
+
+static int lu_failed(const char *what, cudaError_t e)
+{
+  fprintf(stderr, "clp_b200: dense_invert: %s: %s\n", what, cudaGetErrorString(e));
+  return -97;
+}
+#define LU_OK(call, what)                                                                         \
+  do {                                                                                            \
+    const cudaError_t e__ = (call);                                                               \
+    if (e__ != cudaSuccess)                                                                       \
+      return lu_failed(what, e__);                                                                \
+  } while (0)
+
 /* In: A = k x k matrix, column major, leading dimension ld (device).  Out: X = A^-1 (same
-   layout), A is overwritten by its LU factors.  hostIpiv/hostPerm: host scratch of k ints,
-   dIpiv/dPerm/dInfo: device scratch.  Returns 0 or (1 + index of the first column without an
-   acceptable pivot).  Synchronizes the stream once (pivot vector -> permutation). */
-int dense_invert(double *A, double *X, int k, int ld, int *dIpiv, int *dPerm, int *dInfo,
-                 int *hostIpiv, int *hostPerm, double singularTol, cudaStream_t s, int shardW,
-                 int shardRank, int (*allGather)(void *, void *, size_t, void *), void *comm,
+   layout), A is overwritten by its LU factors.  w: scratch reserved for at least k rows.  Returns 0,
+   (1 + index of the first column without an acceptable pivot), or a negative code after one line on
+   stderr when a CUDA call or the all-gather fails.  When it returns 0 or a column, w.hostPerm holds the
+   row permutation composed from the pivots of all k columns.  Synchronizes the stream once (pivot
+   vector -> permutation). */
+int dense_invert(double *A, double *X, int k, int ld, LuWorkspace &w, double singularTol, cudaStream_t s,
+                 int shardW, int shardRank, int (*allGather)(void *, void *, size_t, void *), void *comm,
                  void (*hostOverlap)(void *), void *overlapCtx)
 {
   if (k <= 0)
     return 0;
-  cudaMemsetAsync(dInfo, 0, sizeof(int), s);
-  // scratch of the cooperative panel kernel (allocated once per process)
-  static unsigned long long *pubKey = nullptr;
-  static double *pubRows = nullptr, *pubDiag = nullptr;
-  static unsigned int *barCounter = nullptr;
-  static int numSMs = 0;
-  static int clusterState = getenv("CLPB_NO_CLUSTER_PANEL") ? -1 : 0; // 0 untried, 1 usable, -1 refused
-  static int *permBuf = nullptr;     // composed row permutation of the current panel (lu_perm_kernel)
-  static double *swapTmp = nullptr;  // [2*NB][k] staging of the interchanged rows
-  static size_t swapCap = 0;
-  if ((size_t)k > swapCap) {
-    if (swapTmp)
-      cudaFree(swapTmp);
-    swapCap = (size_t)k + k / 4 + 64;
-    if (cudaMalloc(&swapTmp, sizeof(double) * 2 * NB * swapCap) != cudaSuccess) {
-      swapTmp = nullptr;
-      swapCap = 0;
-      return -99;
-    }
+  if (k > w.maxK || k > w.swapK) {
+    fprintf(stderr, "clp_b200: dense_invert: scratch reserved for %d / %d rows, nucleus of %d\n", w.maxK,
+            w.swapK, k);
+    return -97;
   }
-  if (!permBuf && cudaMalloc(&permBuf, sizeof(int) * (1 + 4 * NB)) != cudaSuccess)
-    return -99;
-  if (!pubKey) {
-    numSMs = device_sm_count();
-    if (cudaMalloc(&pubKey, sizeof(unsigned long long) * NB * numSMs) != cudaSuccess ||
-        cudaMalloc(&pubRows, sizeof(double) * NB * numSMs * NB) != cudaSuccess ||
-        cudaMalloc(&pubDiag, sizeof(double) * NB * NB) != cudaSuccess ||
-        cudaMalloc(&barCounter, sizeof(unsigned int)) != cudaSuccess) {
-      pubKey = nullptr;
-      return -99;
-    }
-    cudaFuncSetAttribute(lu_panel_coop_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         kPanelMaxRowsPerCta * kSlabPitch * (int)sizeof(double));
-  }
-  static int trace = -1;
-  if (trace < 0)
-    trace = getenv("CLPB_REFACTOR_TRACE") ? 1 : 0;
-  cudaEvent_t tev[6];
-  if (trace) {
-    for (auto &e : tev)
-      cudaEventCreate(&e);
-    cudaEventRecord(tev[0], s);
-  }
-  cudaMemsetAsync(barCounter, 0, sizeof(unsigned int), s);
+  // Whether the card grants the 16-CTA non-portable cluster depends on its GPC layout: tried once per
+  // process, and once refused every panel goes to the cooperative kernel.  0 untried, 1 usable, -1 refused.
+  static int clusterState = 0;
+  const int numSMs = device_sm_count();
+  const int maxSmem = kPanelMaxRowsPerCta * kSlabPitch * (int)sizeof(double);
+  cudaGetLastError(); // an error recorded before this call is not one of the factorization's
+  LU_OK(cudaFuncSetAttribute(lu_panel_coop_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, maxSmem),
+        "shared-memory opt-in of lu_panel_coop_kernel");
+  LU_OK(cudaMemsetAsync(w.dInfo, 0, sizeof(int), s), "clearing info");
+  LU_OK(cudaMemsetAsync(w.barrierCounter, 0, sizeof(unsigned int), s), "clearing the barrier counter");
   unsigned int barrierBase = 0;
   for (int j0 = 0; j0 < k; j0 += NB) {
     int nb = k - j0 < NB ? k - j0 : NB;
     const int nrows = k - j0;
-    static int minRows = 0; // rows per CTA of the panel kernel: fewer, fatter CTAs make the per-column grid barrier cheaper
-    if (minRows == 0) {
-      const char *e = getenv("CLPB_PANEL_ROWS");
-      minRows = e ? atoi(e) : 32;
-      if (minRows < 32)
-        minRows = 32;
-    }
-    int G = (nrows + minRows - 1) / minRows;
-    if (G > numSMs)
-      G = numSMs;
-    if (G < 1)
-      G = 1;
-    int R = (nrows + G - 1) / G;
     bool panelDone = false;
     if (clusterState >= 0 && nrows <= kPanelCluster * kPanelMaxRowsPerCta) {
-      // one 16-CTA cluster (non-portable size: opted in once); falls back for good if the launch is refused
+      // one 16-CTA cluster (non-portable size: opted in once)
       const int Rc = (nrows + kPanelCluster - 1) / kPanelCluster;
       const size_t smem = (size_t)Rc * kSlabPitch * sizeof(double);
       if (clusterState == 0) {
         clusterState = 1;
         if (cudaFuncSetAttribute(lu_panel_cluster_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess ||
-            cudaFuncSetAttribute(lu_panel_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 kPanelMaxRowsPerCta * kSlabPitch * (int)sizeof(double)) != cudaSuccess) {
+            cudaFuncSetAttribute(lu_panel_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, maxSmem) != cudaSuccess) {
           cudaGetLastError();
           clusterState = -1;
         }
@@ -750,8 +680,8 @@ int dense_invert(double *A, double *X, int k, int ld, int *dIpiv, int *dPerm, in
         attr.val.clusterDim.z = 1;
         cfg.attrs = &attr;
         cfg.numAttrs = 1;
-        if (cudaLaunchKernelEx(&cfg, lu_panel_cluster_kernel, A, k, ld, j0, nb, Rc, dIpiv, dInfo, singularTol) ==
-            cudaSuccess) {
+        if (cudaLaunchKernelEx(&cfg, lu_panel_cluster_kernel, A, k, ld, j0, nb, Rc, w.dIpiv, w.dInfo,
+                               singularTol) == cudaSuccess) {
           panelDone = true;
         } else {
           cudaGetLastError();
@@ -759,32 +689,34 @@ int dense_invert(double *A, double *X, int k, int ld, int *dIpiv, int *dPerm, in
         }
       }
     }
-    if (panelDone) {
-    } else if (R <= kPanelMaxRowsPerCta) {
-      double *Aarg = A;
-      int karg = k, ldarg = ld, j0arg = j0, nbarg = nb, Rarg = R;
-      double tolarg = singularTol;
-      void *args[] = {&Aarg, &karg, &ldarg, &j0arg, &nbarg, &Rarg, &dIpiv, &dInfo, &tolarg,
-                      &pubKey, &pubRows, &pubDiag, &barCounter, &barrierBase};
-      if (cudaLaunchCooperativeKernel((void *)lu_panel_coop_kernel, dim3(G), dim3(256), args,
-                                      (size_t)R * kSlabPitch * sizeof(double), s) != cudaSuccess) {
-        cudaGetLastError(); // the single-CTA panel kernel does the same work without a grid barrier
-        lu_panel_kernel<<<1, 1024, 0, s>>>(A, k, ld, j0, nb, dIpiv, dInfo, singularTol);
-      } else {
-        barrierBase += (unsigned int)nb * (unsigned int)G;
+    if (!panelDone) {
+      int G = (nrows + kPanelMinRowsPerCta - 1) / kPanelMinRowsPerCta;
+      if (G > numSMs)
+        G = numSMs;
+      int R = (nrows + G - 1) / G;
+      if (R > kPanelMaxRowsPerCta) {
+        // 640 x SMs rows: the nucleus would need 16 k^2 >= 85 GB for Ninv and NinvT, more than any H100 has
+        fprintf(stderr, "clp_b200: dense_invert: a panel of %d rows exceeds the %d x %d rows lu_panel_coop_kernel holds\n",
+                nrows, kPanelMaxRowsPerCta, numSMs);
+        return -97;
       }
-    } else {
-      lu_panel_kernel<<<1, 1024, 0, s>>>(A, k, ld, j0, nb, dIpiv, dInfo, singularTol);
+      void *args[] = {&A,         &k,         &ld,        &j0,       &nb,
+                      &R,         &w.dIpiv,   &w.dInfo,   &singularTol,
+                      &w.pubKey,  &w.pubRows, &w.pubDiag, &w.barrierCounter, &barrierBase};
+      LU_OK(cudaLaunchCooperativeKernel((void *)lu_panel_coop_kernel, dim3(G), dim3(256), args,
+                                        (size_t)R * kSlabPitch * sizeof(double), s),
+            "cooperative launch of lu_panel_coop_kernel");
+      barrierBase += (unsigned int)nb * (unsigned int)G;
     }
     // interchanges on the columns left and right of the panel
     int c0 = j0 + nb;
     {
       const int ncols = j0 + (k - c0);
       if (ncols > 0) {
-        lu_perm_kernel<<<1, 1, 0, s>>>(dIpiv, j0, nb, permBuf);
+        lu_perm_kernel<<<1, 1, 0, s>>>(w.dIpiv, j0, nb, w.panelPerm);
         dim3 grid((ncols + 127) / 128, 2 * NB);
-        lu_swap_gather_kernel<<<grid, 128, 0, s>>>(A, ld, permBuf, j0, c0, ncols, swapTmp);
-        lu_swap_scatter_kernel<<<grid, 128, 0, s>>>(A, ld, permBuf, j0, c0, ncols, swapTmp);
+        lu_swap_gather_kernel<<<grid, 128, 0, s>>>(A, ld, w.panelPerm, j0, c0, ncols, w.swapTmp);
+        lu_swap_scatter_kernel<<<grid, 128, 0, s>>>(A, ld, w.panelPerm, j0, c0, ncols, w.swapTmp);
       }
     }
     if (c0 < k) {
@@ -793,30 +725,31 @@ int dense_invert(double *A, double *X, int k, int ld, int *dIpiv, int *dPerm, in
                A + (size_t)c0 * ld + j0, ld, k - c0, k - c0, nb, s);
     }
   }
+  LU_OK(cudaGetLastError(), "LU launches");
   int info = 0;
-  if (trace)
-    cudaEventRecord(tev[1], s);
-  cudaMemcpyAsync(hostIpiv, dIpiv, sizeof(int) * k, cudaMemcpyDeviceToHost, s);
-  cudaMemcpyAsync(&info, dInfo, sizeof(int), cudaMemcpyDeviceToHost, s);
+  LU_OK(cudaMemcpyAsync(w.hostIpiv, w.dIpiv, sizeof(int) * k, cudaMemcpyDeviceToHost, s), "copying the pivots");
+  LU_OK(cudaMemcpyAsync(&info, w.dInfo, sizeof(int), cudaMemcpyDeviceToHost, s), "copying info");
   if (hostOverlap)
     hostOverlap(overlapCtx); // host work of the caller (S1 of the new basis) while the LU runs
-  cudaStreamSynchronize(s);
-  if (info != 0)
-    return info;
+  LU_OK(cudaStreamSynchronize(s), "LU");
+  // Also for a singular nucleus: the interchange of a column without a pivot is the identity and later
+  // ones never touch its position, so hostPerm[info - 1] is the row the first info - 1 pivots parked there.
   for (int i = 0; i < k; i++)
-    hostPerm[i] = i;
+    w.hostPerm[i] = i;
   for (int j = 0; j < k; j++) {
-    int p = hostIpiv[j];
+    int p = w.hostIpiv[j];
     if (p != j) {
-      int t = hostPerm[j];
-      hostPerm[j] = hostPerm[p];
-      hostPerm[p] = t;
+      int t = w.hostPerm[j];
+      w.hostPerm[j] = w.hostPerm[p];
+      w.hostPerm[p] = t;
     }
   }
-  cudaMemcpyAsync(dPerm, hostPerm, sizeof(int) * k, cudaMemcpyHostToDevice, s);
+  if (info != 0)
+    return info;
+  LU_OK(cudaMemcpyAsync(w.dPerm, w.hostPerm, sizeof(int) * k, cudaMemcpyHostToDevice, s), "copying the permutation");
   {
     size_t total = (size_t)ld * k;
-    set_permuted_identity_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(X, k, ld, dPerm);
+    set_permuted_identity_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(X, k, ld, w.dPerm);
   }
   // Two-level blocking: triangular solves with the NB x NB diagonal blocks, rank-NB updates only
   // inside an outer block of OB columns, one rank-OB update per outer block for the rest (the bulk
@@ -831,27 +764,23 @@ int dense_invert(double *A, double *X, int k, int ld, int *dIpiv, int *dPerm, in
     xc0 = shardRank * perC < k ? shardRank * perC : k;
     xc1 = xc0 + perC < k ? xc0 + perC : k;
   }
-  double *const Xfull = X;
-  const int kfull = k; // rows of X (the substitutions run over all k rows of the column block)
-  X = Xfull + (size_t)xc0 * ld;
-  const int ncol = xc1 - xc0; // columns of this rank
-  // forward: X := L^-1 X
+  double *const Xr = X + (size_t)xc0 * ld; // this rank's columns, all k rows of them
+  const int ncol = xc1 - xc0;
+  // forward: Xr := L^-1 Xr
   for (int J0 = 0; J0 < k; J0 += OB) {
     const int J1 = J0 + OB < k ? J0 + OB : k;
     for (int j0 = J0; j0 < J1; j0 += NB) {
       int nb = J1 - j0 < NB ? J1 - j0 : NB;
       if (ncol > 0)
-        trsm_kernel<<<(ncol + 127) / 128, 128, 0, s>>>(A, ld, X, ld, j0, nb, 0, ncol, true);
+        trsm_kernel<<<(ncol + 127) / 128, 128, 0, s>>>(A, ld, Xr, ld, j0, nb, 0, ncol, true);
       int r0 = j0 + nb;
       if (r0 < J1)
-        gemm_sub(X + r0, ld, A + (size_t)j0 * ld + r0, ld, X + j0, ld, J1 - r0, ncol, nb, s);
+        gemm_sub(Xr + r0, ld, A + (size_t)j0 * ld + r0, ld, Xr + j0, ld, J1 - r0, ncol, nb, s);
     }
     if (J1 < k)
-      gemm_sub(X + J1, ld, A + (size_t)J0 * ld + J1, ld, X + J0, ld, k - J1, ncol, J1 - J0, s);
+      gemm_sub(Xr + J1, ld, A + (size_t)J0 * ld + J1, ld, Xr + J0, ld, k - J1, ncol, J1 - J0, s);
   }
-  if (trace)
-    cudaEventRecord(tev[2], s);
-  // backward: X := U^-1 X
+  // backward: Xr := U^-1 Xr
   const int lastOuter = ((k - 1) / OB) * OB;
   for (int J0 = lastOuter; J0 >= 0; J0 -= OB) {
     const int J1 = J0 + OB < k ? J0 + OB : k;
@@ -859,31 +788,20 @@ int dense_invert(double *A, double *X, int k, int ld, int *dIpiv, int *dPerm, in
     for (int j0 = lastInner; j0 >= J0; j0 -= NB) {
       int nb = J1 - j0 < NB ? J1 - j0 : NB;
       if (ncol > 0)
-        trsm_kernel<<<(ncol + 127) / 128, 128, 0, s>>>(A, ld, X, ld, j0, nb, 0, ncol, false);
+        trsm_kernel<<<(ncol + 127) / 128, 128, 0, s>>>(A, ld, Xr, ld, j0, nb, 0, ncol, false);
       if (j0 > J0)
-        gemm_sub(X + J0, ld, A + (size_t)j0 * ld + J0, ld, X + j0, ld, j0 - J0, ncol, nb, s);
+        gemm_sub(Xr + J0, ld, A + (size_t)j0 * ld + J0, ld, Xr + j0, ld, j0 - J0, ncol, nb, s);
     }
     if (J0 > 0)
-      gemm_sub(X, ld, A + (size_t)J0 * ld, ld, X + J0, ld, J0, ncol, J1 - J0, s);
+      gemm_sub(Xr, ld, A + (size_t)J0 * ld, ld, Xr + J0, ld, J0, ncol, J1 - J0, s);
   }
-  X = Xfull;
-  (void)kfull;
-  if (trace) {
-    cudaEventRecord(tev[3], s);
-    cudaEventSynchronize(tev[3]);
-    float a = 0, b = 0, c = 0;
-    cudaEventElapsedTime(&a, tev[0], tev[1]);
-    cudaEventElapsedTime(&b, tev[1], tev[2]);
-    cudaEventElapsedTime(&c, tev[2], tev[3]);
-    fprintf(stderr, "clp_b200: dense_invert k %d: LU %.2f ms, host sync + forward %.2f ms, backward %.2f ms\n", k, a, b, c);
-    for (auto &e : tev)
-      cudaEventDestroy(e);
-  }
+  LU_OK(cudaGetLastError(), "substitution launches");
   if (shardW > 1 && allGather != nullptr) {
     if (allGather(comm, X, sizeof(double) * (size_t)perC * ld, s) != 0)
       return -98;
   }
   zero_padding_kernel<<<(k + 255) / 256, 256, 0, s>>>(X, k, ld);
+  LU_OK(cudaGetLastError(), "zero_padding_kernel launch");
   return 0;
 }
 

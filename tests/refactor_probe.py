@@ -1,5 +1,5 @@
 """Refactorization time at the C2 bench basis (k ~ 4.7k): CUDA-event ms per refactorization
-(gather + LU + inverse + transpose + host symbolic part), for CLPB_PANEL_ROWS experiments.
+(gather + LU + inverse + transpose + host symbolic part).
   python tests/refactor_probe.py [frequency] [iterations]"""
 import os, sys, json
 sys.path.insert(0, ".")
@@ -17,5 +17,5 @@ for k, v in (("timing", 1), ("factorizationFrequency", freq), ("maximumIteration
 s.dual()
 ph = s.phaseTimes()
 nr = s.numberRefactorizations()
-print(json.dumps({"panel_rows": os.environ.get("CLPB_PANEL_ROWS", "32"), "refactorizations": nr, "nucleus": s.nucleusSize(),
+print(json.dumps({"refactorizations": nr, "nucleus": s.nucleusSize(),
                   "refactor_ms_each": ph["refactor"] / max(1, nr), "iterations": s.numberIterations()}))
