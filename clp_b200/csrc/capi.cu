@@ -346,7 +346,7 @@ int Clpb_denseInvert(int k, const double *a, double *x)
     // nothing between the allocations and the releases throws: every path frees everything
     int info = -99;
     if (cudaMalloc(&dA, bytes) == cudaSuccess && cudaMalloc(&dX, bytes) == cudaSuccess &&
-        clpb::lu_workspace_reserve(w, k, k) == cudaSuccess && cudaStreamCreate(&s) == cudaSuccess &&
+        clpb::lu_workspace_reserve(w, k) == cudaSuccess && cudaStreamCreate(&s) == cudaSuccess &&
         cudaMemset(dA, 0, bytes) == cudaSuccess &&
         // column-major with leading dimension ld
         cudaMemcpy2D(dA, sizeof(double) * ld, a, sizeof(double) * k, sizeof(double) * k, k,

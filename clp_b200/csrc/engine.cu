@@ -422,7 +422,7 @@ int Engine::setupDevice()
   dZ = dalloc<double>(n);
   dObj = dalloc<double>(2);
   dCounters = dalloc<int>(4);
-  CUDA_OK(lu_workspace_reserve(lu, m, 0));
+  CUDA_OK(lu_workspace_reserve(lu, m));
   CUDA_OK(cudaMallocHost(&hState, sizeof(IterState)));
   CUDA_OK(cudaMallocHost(&hRec, sizeof(IterRecord) * d.recCap));
   d.k = 0;
@@ -626,7 +626,6 @@ int Engine::refactor()
     if ((size_t)k * ldk > nucCap) {
       int kc = std::min(m, std::max(k + k / 4 + 64, 256));
       int ldc = roundUp(kc, 8);
-      CUDA_OK(lu_workspace_reserve(lu, m, kc));
       nucCap = (size_t)kc * ldc;
       // the old (smaller) pair is released first: at m = 5e4 a factor pair is up to 40 GB
       for (double *old : {d.Ninv, d.NinvT})
@@ -694,7 +693,9 @@ int Engine::refactor()
                           [](void *c) { (*static_cast<Ctx *>(c)->fn)(); }, &ctx);
       if (info < 0)
         throw std::runtime_error("clp_b200: refactorization failed (CUDA error or collective)");
-      kernelLaunches += 6 * ((k + 31) / 32) * 2;
+      // per 32-column panel: panel, interchange + TRSM, DGEMM; per 32 rows of each substitution: TRSM
+      // and about one DGEMM; plus the identities, the inverse permutation and two transposes
+      kernelLaunches += 7 * ((k + 31) / 32) + 5;
     } else {
       buildS1();
     }
@@ -729,8 +730,6 @@ int Engine::refactor()
       CUDA_OK(cudaMemcpyAsync(dS1cVal, s1cVal.data(), sizeof(double) * s1Start[m], cudaMemcpyHostToDevice, stream));
     }
     if (info == 0) {
-      if (k > 0)
-        launch_transpose(d.Ninv, d.NinvT, k, ldk, stream);
       // weights follow their variables; pivotVariable takes the canonical order
       CUDA_OK(cudaMemcpyAsync(dSrcPos, srcPos.data(), sizeof(int) * m, cudaMemcpyHostToDevice, stream));
       launch_permute_weights(d.weights, dWeightsTmp, dSrcPos, m, stream);

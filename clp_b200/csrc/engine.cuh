@@ -231,28 +231,24 @@ void launch_eta_append_test(const DeviceModel &d, int pivotRow, int seqIn, cudaS
 // Scratch of dense_invert, owned by its caller (one per model): two models never share a buffer or a
 // grid-barrier counter, and dense_invert itself never allocates.
 struct LuWorkspace {
-  int maxK = 0;                          // rows the pivot and permutation buffers hold
-  int *dIpiv = nullptr;                  // [maxK] pivot row of each column
-  int *dPerm = nullptr;                  // [maxK] device copy of hostPerm
+  int maxK = 0;                          // rows the permutation buffers hold
+  int *dPerm = nullptr;                  // [maxK] row permutation, composed on the device panel by panel
+  int *dInvPerm = nullptr;               // [maxK] its inverse
   int *dInfo = nullptr;                  // 1 + first column without an acceptable pivot, or 0
-  int *hostIpiv = nullptr;               // [maxK] host copies (pageable)
-  int *hostPerm = nullptr;
+  int *hostPerm = nullptr;               // [maxK] host copy of dPerm (pageable)
   unsigned long long *pubKey = nullptr;  // cooperative panel kernel: candidate key per column and CTA,
   double *pubRows = nullptr;             //   candidate row per column and CTA,
   double *pubDiag = nullptr;             //   diagonal row per column,
   unsigned int *barrierCounter = nullptr; //  grid-barrier arrival counter
-  int *panelPerm = nullptr;              // interchanges of the current panel composed (lu_perm_kernel)
-  double *swapTmp = nullptr;             // [2 x 32][swapK] staging of the interchanged rows
-  int swapK = 0;
+  int *panelPerm = nullptr;              // interchanges of the current panel composed (by the panel kernel)
 };
-// Allocates what is missing and grows what is smaller than asked: pivots for maxK rows, staging for
-// nuclei of up to swapK.  On failure everything is released and the error is returned.
-cudaError_t lu_workspace_reserve(LuWorkspace &w, int maxK, int swapK);
+// Allocates what is missing and grows what is smaller than asked: permutations for maxK rows.  On
+// failure everything is released and the error is returned.
+cudaError_t lu_workspace_reserve(LuWorkspace &w, int maxK);
 void lu_workspace_release(LuWorkspace &w); // any state, also empty or released
 int dense_invert(double *A, double *X, int k, int ld, LuWorkspace &w, double singularTol,
                  cudaStream_t s, int shardW = 1, int shardRank = 0,
                  int (*allGather)(void *, void *, size_t, void *) = nullptr, void *comm = nullptr,
                  void (*hostOverlap)(void *) = nullptr, void *overlapCtx = nullptr);
-void launch_transpose(const double *src, double *dst, int k, int ld, cudaStream_t s);
 
 } // namespace clpb

@@ -178,7 +178,7 @@ private:
   int currentCycle = 0;                  // refactorization interval in force (adapted from the drift)
   int *dSrcPos = nullptr, *dCounters = nullptr;
   unsigned char *dFlipFlag = nullptr;
-  LuWorkspace lu; // scratch of dense_invert; its staging buffer grows with nucCap
+  LuWorkspace lu; // scratch of dense_invert
   int *dS1RowStart = nullptr, *dS1Col = nullptr;
   double *dS1Val = nullptr;
   int *dS1cStart = nullptr, *dS1cRow = nullptr;

@@ -7,8 +7,9 @@
 //
 // The k x k nucleus (structural basic columns restricted to rows whose slack is nonbasic) is
 // LU-factorized with partial pivoting by a blocked right-looking algorithm (panel kernel +
-// row swaps + unit-lower TRSM + rank-NB DGEMM update) and the factors are then turned into
-// the explicit inverse X = U^-1 L^-1 P by blocked forward/backward substitution (TRSM + DGEMM).
+// fused row interchanges and unit-lower TRSM + rank-NB DGEMM update) and the factors are then turned
+// into the explicit inverse X = U^-1 L^-1 P by blocked forward/backward substitution of the identity
+// (TRSM + DGEMM) and a permuted transpose.
 // Everything is fp64 FMA; the matrix is column major with leading dimension ld.
 #include "engine.cuh"
 
@@ -51,10 +52,53 @@ __device__ __forceinline__ void grid_barrier(unsigned int *counter, unsigned int
   __syncthreads();
 }
 
+// The nb interchanges (j0 + jj <-> piv[jj]) of a panel composed into one row permutation, by one warp
+// at the end of the panel kernel.  perm[1 + l] is the row whose content ends in panel row j0 + l; the
+// rows below the panel that some interchange touched are perm[1 + NB + t], t < perm[0], and their
+// content comes from panel row perm[1 + 2*NB + t] (a pivot row only ever receives the current content
+// of a panel row, and panel rows only ever hold original panel rows or pivot rows).
+__device__ __forceinline__ void compose_panel_perm(const int *__restrict__ piv, int j0, int nb,
+                                                   int *__restrict__ perm)
+{
+  const int lane = threadIdx.x & 31;
+  int cur = j0 + lane, outRow = -1, outSrc = j0, nOut = 0;
+  for (int jj = 0; jj < nb; jj++) {
+    const int p = piv[jj];
+    if (p == j0 + jj)
+      continue;
+    const int a = __shfl_sync(0xffffffffu, cur, jj);
+    if (p - j0 < nb) {
+      const int b = __shfl_sync(0xffffffffu, cur, p - j0);
+      if (lane == jj)
+        cur = b;
+      if (lane == p - j0)
+        cur = a;
+    } else {
+      const unsigned int hit = __ballot_sync(0xffffffffu, outRow == p);
+      const int t = hit ? __ffs(hit) - 1 : nOut++;
+      const int b = hit ? __shfl_sync(0xffffffffu, outSrc, t) : p;
+      if (lane == jj)
+        cur = b;
+      if (lane == t) {
+        outRow = p;
+        outSrc = a;
+      }
+    }
+  }
+  if (lane < nb)
+    perm[1 + lane] = cur;
+  if (lane < nOut) {
+    perm[1 + NB + lane] = outRow;
+    perm[1 + 2 * NB + lane] = outSrc;
+  }
+  if (lane == 0)
+    perm[0] = nOut;
+}
+
 // rows [j0 + cta*R, j0 + (cta+1)*R) of the panel belong to CTA 'cta'
 __global__ void __launch_bounds__(256)
     lu_panel_coop_kernel(double *__restrict__ A, int k, int ld, int j0, int nb, int R,
-                         int *__restrict__ ipiv, int *__restrict__ info, double singularTol,
+                         int *__restrict__ panelPerm, int *__restrict__ info, double singularTol,
                          unsigned long long *__restrict__ pubKey, double *__restrict__ pubRows,
                          double *__restrict__ pubDiag, unsigned int *__restrict__ barrierCounter,
                          unsigned int barrierBase)
@@ -62,6 +106,7 @@ __global__ void __launch_bounds__(256)
   extern __shared__ double slab[]; // [R][kSlabPitch]
   __shared__ unsigned long long sBest[8];
   __shared__ int sWinCta[8];
+  __shared__ int sPiv[NB];
   __shared__ double urow[NB];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int G = gridDim.x, cta = blockIdx.x;
@@ -143,11 +188,10 @@ __global__ void __launch_bounds__(256)
     const double pivAbs = __longlong_as_double((long long)(wkey & ~0xFFFFFull));
     const int piv = j0 + (0xFFFFF - (int)(wkey & 0xFFFFFull)); // global pivot row
     const bool singular = (wkey == 0ull) || !(pivAbs >= singularTol);
-    if (cta == 0 && tid == 0) {
-      ipiv[j] = singular ? j : piv;
-      if (singular && *info == 0)
-        *info = j + 1;
-    }
+    if (tid == 0)
+      sPiv[jj] = singular ? j : piv;
+    if (cta == 0 && tid == 0 && singular && *info == 0)
+      *info = j + 1;
     if (singular) {
       __syncthreads();
       continue; // uniform across the grid: leave the column, the caller repairs the basis
@@ -179,26 +223,33 @@ __global__ void __launch_bounds__(256)
   for (int c = 0; c < nb; c++)
     for (int q = tid; q < rowsLocal; q += 256)
       A[(size_t)(j0 + c) * ld + r0 + q] = slab[q * kSlabPitch + c];
+  if (cta == 0 && warp == 0)
+    compose_panel_perm(sPiv, j0, nb, panelPerm);
 }
 
 // ---- the same panel on ONE thread-block cluster (16 CTAs of one GPC, distributed shared memory).
 // The per-column pivot exchange of lu_panel_coop_kernel costs a grid barrier plus two dependent L2 round
-// trips; inside a cluster the candidate
-// keys, the pivot row and the diagonal row are read straight out of the peers' shared memory and the two
-// synchronisations are hardware cluster barriers.  Panels of up to 16 x kPanelMaxRowsPerCta rows.
+// trips; inside a cluster it costs ONE hardware cluster barrier per column.  Before it every CTA copies
+// its candidate key and row (and the owner of the diagonal row that row) into a publication slot in its
+// own shared memory; after it every CTA reads the winner's row and the diagonal row out of the peers'
+// slots and swaps and eliminates locally.  The slots are double-buffered by column parity: slot jj & 1
+// is rewritten at column jj + 2, after every peer has passed the barrier of column jj + 1 and so has
+// finished reading it.  Panels of up to 16 x kPanelMaxRowsPerCta rows.
 constexpr int kPanelCluster = 16;
 
 __global__ void __launch_bounds__(256)
     lu_panel_cluster_kernel(double *__restrict__ A, int k, int ld, int j0, int nb, int R,
-                            int *__restrict__ ipiv, int *__restrict__ info, double singularTol)
+                            int *__restrict__ panelPerm, int *__restrict__ info, double singularTol)
 {
   namespace cg = cooperative_groups;
   cg::cluster_group cluster = cg::this_cluster();
-  extern __shared__ double slab[]; // [R][kSlabPitch], same offset in every CTA of the cluster
+  extern __shared__ double slab[]; // [R][kSlabPitch]
   __shared__ unsigned long long sBest[8];
-  __shared__ unsigned long long sKey;  // this CTA's candidate of the current column
   __shared__ unsigned long long sWin;
+  __shared__ int sPiv[NB];
   __shared__ double urow[NB], drow[NB];
+  __shared__ unsigned long long slotKey[2];      // publication slots, same offset in every CTA
+  __shared__ double slotRow[2][NB], slotDiag[2][NB];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int cta = (int)cluster.block_rank();
   const int r0 = j0 + cta * R;
@@ -208,7 +259,7 @@ __global__ void __launch_bounds__(256)
       slab[q * kSlabPitch + c] = A[(size_t)(j0 + c) * ld + r0 + q];
   __syncthreads();
   for (int jj = 0; jj < nb; jj++) {
-    const int j = j0 + jj;
+    const int j = j0 + jj, par = jj & 1;
     const int ownerJ = (j - j0) / R;
     unsigned long long best = 0ull;
     for (int q = tid; q < rowsLocal; q += 256) {
@@ -224,52 +275,51 @@ __global__ void __launch_bounds__(256)
       best = max(best, __shfl_xor_sync(0xffffffffu, best, o));
     if (lane == 0)
       sBest[warp] = best;
-    __syncthreads();
-    if (tid == 0) {
-      unsigned long long cand = 0ull;
+    __syncthreads(); // also: the elimination of the previous column is complete
+    unsigned long long cand = 0ull;
 #pragma unroll
-      for (int w = 0; w < 8; w++)
-        cand = max(cand, sBest[w]);
-      sKey = cand;
-    }
-    cluster.sync(); // every CTA's candidate is published
+    for (int w = 0; w < 8; w++)
+      cand = max(cand, sBest[w]);
+    if (tid == 0)
+      slotKey[par] = cand;
+    if (cand != 0ull && tid < NB)
+      slotRow[par][tid] = slab[(j0 + (0xFFFFF - (int)(cand & 0xFFFFFull)) - r0) * kSlabPitch + tid];
+    if (ownerJ == cta && tid < NB)
+      slotDiag[par][tid] = slab[(j - r0) * kSlabPitch + tid];
+    cluster.sync(); // every CTA's slot of this column is published
     if (warp == 0) {
       unsigned long long v = 0ull;
       if (lane < kPanelCluster)
-        v = *cluster.map_shared_rank(&sKey, lane);
+        v = *cluster.map_shared_rank(&slotKey[par], lane);
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1)
         v = max(v, __shfl_xor_sync(0xffffffffu, v, o));
       if (lane == 0)
         sWin = v;
+      if (v != 0ull) { // pivot row out of the winner's slot, diagonal row out of its owner's
+        const int ownerP = (0xFFFFF - (int)(v & 0xFFFFFull)) / R;
+        urow[lane] = *cluster.map_shared_rank(&slotRow[par][lane], ownerP);
+        drow[lane] = *cluster.map_shared_rank(&slotDiag[par][lane], ownerJ);
+      }
     }
     __syncthreads();
     const unsigned long long wkey = sWin;
     const double pivAbs = __longlong_as_double((long long)(wkey & ~0xFFFFFull));
     const int piv = j0 + (0xFFFFF - (int)(wkey & 0xFFFFFull));
     const bool singular = (wkey == 0ull) || !(pivAbs >= singularTol);
-    if (cta == 0 && tid == 0) {
-      ipiv[j] = singular ? j : piv;
-      if (singular && *info == 0)
-        *info = j + 1;
-    }
-    if (singular) {
-      cluster.sync(); // keep the barrier count uniform
-      continue;
-    }
+    if (tid == 0)
+      sPiv[jj] = singular ? j : piv;
+    if (cta == 0 && tid == 0 && singular && *info == 0)
+      *info = j + 1;
+    if (singular)
+      continue; // one barrier per column on both paths: the count stays uniform across the cluster
     const int ownerP = (piv - j0) / R;
-    if (tid < NB) { // pivot row and diagonal row out of their owners' slabs (distributed shared memory)
-      const double *ps = cluster.map_shared_rank(slab, ownerP);
-      const double *ds = cluster.map_shared_rank(slab, ownerJ);
-      urow[tid] = ps[(piv - (j0 + ownerP * R)) * kSlabPitch + tid];
-      drow[tid] = ds[(j - (j0 + ownerJ * R)) * kSlabPitch + tid];
+    if (tid < NB) { // exchange: the old diagonal row moves to row piv, the pivot row moves to row j
+      if (piv != j && ownerP == cta)
+        slab[(piv - r0) * kSlabPitch + tid] = drow[tid];
+      if (ownerJ == cta)
+        slab[(j - r0) * kSlabPitch + tid] = urow[tid];
     }
-    cluster.sync(); // everybody holds both rows: the owners may overwrite them now
-    if (piv != j && ownerP == cta && tid < NB)
-      slab[(piv - r0) * kSlabPitch + tid] = drow[tid];
-    __syncthreads();
-    if (ownerJ == cta && tid < NB)
-      slab[(j - r0) * kSlabPitch + tid] = urow[tid];
     __syncthreads();
     const double inv = 1.0 / urow[jj];
     for (int q = tid; q < rowsLocal; q += 256) {
@@ -281,92 +331,109 @@ __global__ void __launch_bounds__(256)
           r[c] = fma(-l, urow[c], r[c]);
       }
     }
-    __syncthreads();
   }
   cluster.sync(); // nobody exits while a peer may still read its shared memory
   for (int c = 0; c < nb; c++)
     for (int q = tid; q < rowsLocal; q += 256)
       A[(size_t)(j0 + c) * ld + r0 + q] = slab[q * kSlabPitch + c];
+  if (cta == 0 && warp == 0)
+    compose_panel_perm(sPiv, j0, nb, panelPerm);
 }
 
-// Row interchanges of a panel applied to the columns left and right of it.  The nb interchanges touch
-// at most 2*nb rows; lu_perm_kernel composes them into ONE permutation of those rows (perm[0] = count,
-// perm[1+i] = touched row, perm[1+2*NB+i] = the row its final content comes from).  The elements are
-// then moved by two fully parallel kernels through a scratch buffer -- one thread per (column, touched
-// row): gather tmp[i][c] = A[from_i][c], scatter A[row_i][c] = tmp[i][c].  (One thread per column doing
-// its 2*nb strided loads serially left the GPU idle.)
-__global__ void lu_perm_kernel(const int *__restrict__ ipiv, int j0, int nb, int *__restrict__ perm)
+// The panel's composed row permutation (compose_panel_perm) applied to one column of the rows outside
+// the panel's own columns; the warp holds the <= 2*NB touched rows in registers.  Returns the new value
+// of panel row j0 + lane (lane < nb); the touched rows below the panel are written here.
+template <typename T>
+__device__ __forceinline__ T interchange_column(T *__restrict__ col, int j0, int nb, int src, int nOut, int outRow,
+                                                int outSrc)
 {
-  int *rows = perm + 1, *from = perm + 1 + 2 * NB;
-  int n = 0;
-  for (int jj = 0; jj < nb; jj++) {
-    const int j = j0 + jj, p = ipiv[j];
-    if (p == j)
-      continue;
-    int a = -1, b = -1;
-    for (int i = 0; i < n; i++) {
-      if (rows[i] == j)
-        a = i;
-      if (rows[i] == p)
-        b = i;
-    }
-    if (a < 0) {
-      a = n++;
-      rows[a] = j;
-      from[a] = j;
-    }
-    if (b < 0) {
-      b = n++;
-      rows[b] = p;
-      from[b] = p;
-    }
-    const int t = from[a];
-    from[a] = from[b];
-    from[b] = t;
+  const int lane = threadIdx.x & 31;
+  const T orig = lane < nb ? col[j0 + lane] : T(0);
+  const bool inPanel = src - j0 < nb;
+  const T fromPanel = __shfl_sync(0xffffffffu, orig, inPanel ? src - j0 : 0);
+  const T x = inPanel ? fromPanel : col[src];
+  const T toOut = __shfl_sync(0xffffffffu, orig, outSrc - j0);
+  __syncwarp(); // every load of the column is done before a touched row is overwritten
+  if (lane < nOut)
+    col[outRow] = toOut;
+  return x;
+}
+
+// Row interchanges of a panel on the columns left and right of it, and the unit-lower solve with the
+// panel's L11 on the columns right of it, one warp per column; warp ncols applies the interchanges to
+// the row permutation rowPerm of the whole factorization.  Columns are indexed linearly over
+// [0, j0) U [j0 + nb, k).  Lane i holds row i of L11 and sweeps l ascending, which is trsm_kernel's
+// s = fma(-T[i][l], x[l], s) order.
+__global__ void __launch_bounds__(256)
+    lu_interchange_trsm_kernel(double *__restrict__ A, int k, int ld, int j0, int nb,
+                               const int *__restrict__ perm, int *__restrict__ rowPerm)
+{
+  __shared__ double L11[NB][NB + 1];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int c0 = j0 + nb, ncols = j0 + (k - c0);
+  for (int e = threadIdx.x; e < NB * NB; e += blockDim.x) {
+    const int i = e % NB, l = e / NB;
+    L11[i][l] = (i < nb && l < nb) ? A[(size_t)(j0 + l) * ld + j0 + i] : 0.0;
   }
-  perm[0] = n;
+  const int nOut = perm[0];
+  const int src = lane < nb ? perm[1 + lane] : j0;
+  const int outRow = lane < nOut ? perm[1 + NB + lane] : 0;
+  const int outSrc = lane < nOut ? perm[1 + 2 * NB + lane] : j0;
+  __syncthreads();
+  double t[NB];
+#pragma unroll
+  for (int l = 0; l < NB; l++)
+    t[l] = L11[lane][l];
+  for (int q = blockIdx.x * 8 + warp; q <= ncols; q += gridDim.x * 8) {
+    if (q == ncols) {
+      const int v = interchange_column(rowPerm, j0, nb, src, nOut, outRow, outSrc);
+      if (lane < nb)
+        rowPerm[j0 + lane] = v;
+      continue;
+    }
+    const int c = q < j0 ? q : q - j0 + c0;
+    double *col = A + (size_t)c * ld;
+    double x = interchange_column(col, j0, nb, src, nOut, outRow, outSrc);
+    if (c >= c0) {
+#pragma unroll
+      for (int l = 0; l < NB - 1; l++) {
+        const double xl = __shfl_sync(0xffffffffu, x, l);
+        if (lane > l)
+          x = fma(-t[l], xl, x);
+      }
+    }
+    if (lane < nb)
+      col[j0 + lane] = x;
+  }
 }
-// columns are indexed linearly over [0, left) U [right0, right0 + nright)
-__global__ void __launch_bounds__(128)
-    lu_swap_gather_kernel(const double *__restrict__ A, int ld, const int *__restrict__ perm, int left,
-                          int right0, int ncols, double *__restrict__ tmp)
+
+__global__ void iota_kernel(int *__restrict__ v, int k)
 {
-  const int i = blockIdx.y;
-  if (i >= perm[0])
-    return;
-  const int q = blockIdx.x * blockDim.x + threadIdx.x;
-  if (q >= ncols)
-    return;
-  const int c = q < left ? q : q - left + right0;
-  tmp[(size_t)i * ncols + q] = A[(size_t)c * ld + perm[1 + 2 * NB + i]];
-}
-__global__ void __launch_bounds__(128)
-    lu_swap_scatter_kernel(double *__restrict__ A, int ld, const int *__restrict__ perm, int left,
-                           int right0, int ncols, const double *__restrict__ tmp)
-{
-  const int i = blockIdx.y;
-  if (i >= perm[0])
-    return;
-  const int q = blockIdx.x * blockDim.x + threadIdx.x;
-  if (q >= ncols)
-    return;
-  if (perm[1 + i] == perm[1 + 2 * NB + i])
-    return;
-  const int c = q < left ? q : q - left + right0;
-  A[(size_t)c * ld + perm[1 + i]] = tmp[(size_t)i * ncols + q];
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < k)
+    v[i] = i;
 }
 
 // B[j0..j0+nb, c] := T^-1 B[.., c] for columns c in [c0,c1); T = nb x nb triangle of A at (j0,j0)
 //   lower=true : unit lower triangular (forward substitution)
 //   lower=false: upper triangular with diagonal (backward substitution)
-__global__ void __launch_bounds__(128)
+//   BS threads per CTA; the triangle is loaded with all of a thread's loads in flight at once
+template <int BS>
+__global__ void __launch_bounds__(BS)
     trsm_kernel(const double *__restrict__ A, int lda, double *__restrict__ B, int ldb, int j0,
                 int nb, int c0, int c1, bool lower)
 {
   __shared__ double T[NB][NB + 1];
-  for (int e = threadIdx.x; e < NB * NB; e += blockDim.x) {
-    int i = e % NB, l = e / NB;
-    T[i][l] = (i < nb && l < nb) ? A[(size_t)(j0 + l) * lda + j0 + i] : (i == l ? 1.0 : 0.0);
+  double t[NB * NB / BS];
+#pragma unroll
+  for (int u = 0; u < NB * NB / BS; u++) {
+    const int e = threadIdx.x + u * BS, i = e % NB, l = e / NB;
+    t[u] = (i < nb && l < nb) ? A[(size_t)(j0 + l) * lda + j0 + i] : (i == l ? 1.0 : 0.0);
+  }
+#pragma unroll
+  for (int u = 0; u < NB * NB / BS; u++) {
+    const int e = threadIdx.x + u * BS;
+    T[e % NB][e / NB] = t[u];
   }
   __syncthreads();
   int c = c0 + blockIdx.x * blockDim.x + threadIdx.x;
@@ -498,12 +565,14 @@ bool blas_ready()
 }
 } // namespace
 
+// cuBLAS from M x Nsel >= 256^2 on: the forward substitution passes its full column count, so the choice
+// (and with it the rounding) of an element does not depend on how many columns a step updates
 static void gemm_sub(double *C, int ldc, const double *A, int lda, const double *B, int ldb, int M,
-                     int N, int K, cudaStream_t s)
+                     int N, int K, cudaStream_t s, int Nsel = 0)
 {
   if (M <= 0 || N <= 0 || K <= 0)
     return;
-  if ((long)M * N >= 256L * 256L && blas_ready()) {
+  if ((long)M * (Nsel > 0 ? Nsel : N) >= 256L * 256L && blas_ready()) {
     const double minusOne = -1.0, one = 1.0;
     p_setStream(g_blas, s);
     if (p_dgemm(g_blas, 0 /* N */, 0 /* N */, M, N, K, &minusOne, A, lda, B, ldb, &one, C, ldc) == 0)
@@ -513,26 +582,31 @@ static void gemm_sub(double *C, int ldc, const double *A, int lda, const double 
   gemm_sub_kernel<<<grid, 256, 0, s>>>(C, ldc, A, lda, B, ldb, M, N, K);
 }
 
-__global__ void set_permuted_identity_kernel(double *__restrict__ X, int k, int ld,
-                                             const int *__restrict__ perm)
+__global__ void set_identity_kernel(double *__restrict__ X, int k, int ld)
 {
-  // X = P : row i of P has its one in column perm[i]
   size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   size_t total = (size_t)ld * k;
   if (idx >= total)
     return;
-  int i = (int)(idx % ld), c = (int)(idx / ld);
-  X[idx] = (i < k && perm[i] == c) ? 1.0 : 0.0;
+  X[idx] = (idx % ld == idx / ld) ? 1.0 : 0.0;
 }
 
+__global__ void invert_perm_kernel(const int *__restrict__ perm, int *__restrict__ inv, int k)
+{
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < k)
+    inv[perm[i]] = i;
+}
+
+// dst = src^T with its rows [k, ld) zero; with colMap, column y of src is read from column colMap[y]
 __global__ void transpose_kernel(const double *__restrict__ src, double *__restrict__ dst, int k,
-                                 int ld)
+                                 int ld, const int *__restrict__ colMap)
 {
   __shared__ double tile[32][33];
   int x = blockIdx.x * 32 + threadIdx.x, y0 = blockIdx.y * 32;
   for (int r = threadIdx.y; r < 32; r += 8) {
     int y = y0 + r;
-    tile[r][threadIdx.x] = (x < k && y < k) ? src[(size_t)y * ld + x] : 0.0;
+    tile[r][threadIdx.x] = (x < k && y < k) ? src[(size_t)(colMap ? colMap[y] : y) * ld + x] : 0.0;
   }
   __syncthreads();
   int xo = blockIdx.y * 32 + threadIdx.x, yo0 = blockIdx.x * 32;
@@ -542,25 +616,13 @@ __global__ void transpose_kernel(const double *__restrict__ src, double *__restr
       dst[(size_t)yo * ld + xo] = (xo < k) ? tile[threadIdx.x][r] : 0.0;
   }
 }
-void launch_transpose(const double *src, double *dst, int k, int ld, cudaStream_t s)
+static void launch_transpose(const double *src, double *dst, int k, int ld, const int *colMap, cudaStream_t s)
 {
-  if (k <= 0)
-    return;
   dim3 grid((ld + 31) / 32, (k + 31) / 32);
-  transpose_kernel<<<grid, dim3(32, 8), 0, s>>>(src, dst, k, ld);
+  transpose_kernel<<<grid, dim3(32, 8), 0, s>>>(src, dst, k, ld, colMap);
 }
 
-// zero the padding columns/rows [k, ld) of every row so GEMVs can run over ld
-__global__ void zero_padding_kernel(double *__restrict__ M, int k, int ld)
-{
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= k)
-    return;
-  for (int j = k; j < ld; j++)
-    M[(size_t)i * ld + j] = 0.0;
-}
-
-cudaError_t lu_workspace_reserve(LuWorkspace &w, int maxK, int swapK)
+cudaError_t lu_workspace_reserve(LuWorkspace &w, int maxK)
 {
   cudaError_t e = cudaSuccess;
   auto dev = [&e](auto *&p, size_t count) {
@@ -573,28 +635,20 @@ cudaError_t lu_workspace_reserve(LuWorkspace &w, int maxK, int swapK)
     dev(w.pubRows, NB * sms * NB);
     dev(w.pubDiag, NB * NB);
     dev(w.barrierCounter, 1);
-    dev(w.panelPerm, 1 + 4 * NB);
+    dev(w.panelPerm, 1 + 3 * NB);
     dev(w.dInfo, 1);
   }
   if (maxK > w.maxK) {
-    cudaFree(w.dIpiv);
     cudaFree(w.dPerm);
-    free(w.hostIpiv);
+    cudaFree(w.dInvPerm);
     free(w.hostPerm);
-    w.dIpiv = w.dPerm = w.hostIpiv = w.hostPerm = nullptr;
-    dev(w.dIpiv, maxK);
+    w.dPerm = w.dInvPerm = w.hostPerm = nullptr;
     dev(w.dPerm, maxK);
-    w.hostIpiv = (int *)malloc(sizeof(int) * maxK);
+    dev(w.dInvPerm, maxK);
     w.hostPerm = (int *)malloc(sizeof(int) * maxK);
-    if (e == cudaSuccess && (!w.hostIpiv || !w.hostPerm))
+    if (e == cudaSuccess && !w.hostPerm)
       e = cudaErrorMemoryAllocation;
     w.maxK = maxK;
-  }
-  if (swapK > w.swapK) {
-    cudaFree(w.swapTmp);
-    w.swapTmp = nullptr;
-    dev(w.swapTmp, (size_t)2 * NB * swapK);
-    w.swapK = swapK;
   }
   if (e != cudaSuccess)
     lu_workspace_release(w);
@@ -603,10 +657,9 @@ cudaError_t lu_workspace_reserve(LuWorkspace &w, int maxK, int swapK)
 
 void lu_workspace_release(LuWorkspace &w)
 {
-  for (void *p : {(void *)w.dIpiv, (void *)w.dPerm, (void *)w.dInfo, (void *)w.pubKey, (void *)w.pubRows,
-                  (void *)w.pubDiag, (void *)w.barrierCounter, (void *)w.panelPerm, (void *)w.swapTmp})
+  for (void *p : {(void *)w.dPerm, (void *)w.dInvPerm, (void *)w.dInfo, (void *)w.pubKey, (void *)w.pubRows,
+                  (void *)w.pubDiag, (void *)w.barrierCounter, (void *)w.panelPerm})
     cudaFree(p);
-  free(w.hostIpiv);
   free(w.hostPerm);
   w = LuWorkspace{};
 }
@@ -623,21 +676,21 @@ static int lu_failed(const char *what, cudaError_t e)
       return lu_failed(what, e__);                                                                \
   } while (0)
 
-/* In: A = k x k matrix, column major, leading dimension ld (device).  Out: X = A^-1 (same
-   layout), A is overwritten by its LU factors.  w: scratch reserved for at least k rows.  Returns 0,
-   (1 + index of the first column without an acceptable pivot), or a negative code after one line on
-   stderr when a CUDA call or the all-gather fails.  When it returns 0 or a column, w.hostPerm holds the
-   row permutation composed from the pivots of all k columns.  Synchronizes the stream once (pivot
-   vector -> permutation). */
+/* In: A = k x k matrix, column major, leading dimension ld (device).  Out: X = A^-1 and A = X^T (same
+   layout, rows [k, ld) of both zero).  w: scratch reserved for at least k rows.  Returns 0, (1 + index of
+   the first column without an acceptable pivot), or a negative code after one line on stderr when a CUDA
+   call or the all-gather fails.  When it returns 0 or a column, w.hostPerm holds the row permutation
+   composed from the pivots of all k columns; after a column, A and X hold garbage.  The LU, the
+   substitutions and the transposes are enqueued without a host round trip; hostOverlap runs while they
+   execute, and the stream is synchronized once, at the end. */
 int dense_invert(double *A, double *X, int k, int ld, LuWorkspace &w, double singularTol, cudaStream_t s,
                  int shardW, int shardRank, int (*allGather)(void *, void *, size_t, void *), void *comm,
                  void (*hostOverlap)(void *), void *overlapCtx)
 {
   if (k <= 0)
     return 0;
-  if (k > w.maxK || k > w.swapK) {
-    fprintf(stderr, "clp_b200: dense_invert: scratch reserved for %d / %d rows, nucleus of %d\n", w.maxK,
-            w.swapK, k);
+  if (k > w.maxK) {
+    fprintf(stderr, "clp_b200: dense_invert: scratch reserved for %d rows, nucleus of %d\n", w.maxK, k);
     return -97;
   }
   // Whether the card grants the 16-CTA non-portable cluster depends on its GPC layout: tried once per
@@ -650,6 +703,7 @@ int dense_invert(double *A, double *X, int k, int ld, LuWorkspace &w, double sin
         "shared-memory opt-in of lu_panel_coop_kernel");
   LU_OK(cudaMemsetAsync(w.dInfo, 0, sizeof(int), s), "clearing info");
   LU_OK(cudaMemsetAsync(w.barrierCounter, 0, sizeof(unsigned int), s), "clearing the barrier counter");
+  iota_kernel<<<(k + 255) / 256, 256, 0, s>>>(w.dPerm, k);
   unsigned int barrierBase = 0;
   for (int j0 = 0; j0 < k; j0 += NB) {
     int nb = k - j0 < NB ? k - j0 : NB;
@@ -680,7 +734,7 @@ int dense_invert(double *A, double *X, int k, int ld, LuWorkspace &w, double sin
         attr.val.clusterDim.z = 1;
         cfg.attrs = &attr;
         cfg.numAttrs = 1;
-        if (cudaLaunchKernelEx(&cfg, lu_panel_cluster_kernel, A, k, ld, j0, nb, Rc, w.dIpiv, w.dInfo,
+        if (cudaLaunchKernelEx(&cfg, lu_panel_cluster_kernel, A, k, ld, j0, nb, Rc, w.panelPerm, w.dInfo,
                                singularTol) == cudaSuccess) {
           panelDone = true;
         } else {
@@ -700,64 +754,41 @@ int dense_invert(double *A, double *X, int k, int ld, LuWorkspace &w, double sin
                 nrows, kPanelMaxRowsPerCta, numSMs);
         return -97;
       }
-      void *args[] = {&A,         &k,         &ld,        &j0,       &nb,
-                      &R,         &w.dIpiv,   &w.dInfo,   &singularTol,
-                      &w.pubKey,  &w.pubRows, &w.pubDiag, &w.barrierCounter, &barrierBase};
+      void *args[] = {&A,         &k,           &ld,        &j0,       &nb,
+                      &R,         &w.panelPerm, &w.dInfo,   &singularTol,
+                      &w.pubKey,  &w.pubRows,   &w.pubDiag, &w.barrierCounter, &barrierBase};
       LU_OK(cudaLaunchCooperativeKernel((void *)lu_panel_coop_kernel, dim3(G), dim3(256), args,
                                         (size_t)R * kSlabPitch * sizeof(double), s),
             "cooperative launch of lu_panel_coop_kernel");
       barrierBase += (unsigned int)nb * (unsigned int)G;
     }
-    // interchanges on the columns left and right of the panel
-    int c0 = j0 + nb;
+    // interchanges on the columns left and right of the panel (and on dPerm), L11^-1 on the right ones
+    const int c0 = j0 + nb;
     {
-      const int ncols = j0 + (k - c0);
-      if (ncols > 0) {
-        lu_perm_kernel<<<1, 1, 0, s>>>(w.dIpiv, j0, nb, w.panelPerm);
-        dim3 grid((ncols + 127) / 128, 2 * NB);
-        lu_swap_gather_kernel<<<grid, 128, 0, s>>>(A, ld, w.panelPerm, j0, c0, ncols, w.swapTmp);
-        lu_swap_scatter_kernel<<<grid, 128, 0, s>>>(A, ld, w.panelPerm, j0, c0, ncols, w.swapTmp);
-      }
+      const int warps = j0 + (k - c0) + 1;
+      int blocks = (warps + 7) / 8;
+      if (blocks > 4 * numSMs)
+        blocks = 4 * numSMs;
+      lu_interchange_trsm_kernel<<<blocks, 256, 0, s>>>(A, k, ld, j0, nb, w.panelPerm, w.dPerm);
     }
-    if (c0 < k) {
-      trsm_kernel<<<(k - c0 + 127) / 128, 128, 0, s>>>(A, ld, A, ld, j0, nb, c0, k, true);
+    if (c0 < k)
       gemm_sub(A + (size_t)c0 * ld + c0, ld, A + (size_t)j0 * ld + c0, ld,
                A + (size_t)c0 * ld + j0, ld, k - c0, k - c0, nb, s);
-    }
   }
   LU_OK(cudaGetLastError(), "LU launches");
-  int info = 0;
-  LU_OK(cudaMemcpyAsync(w.hostIpiv, w.dIpiv, sizeof(int) * k, cudaMemcpyDeviceToHost, s), "copying the pivots");
-  LU_OK(cudaMemcpyAsync(&info, w.dInfo, sizeof(int), cudaMemcpyDeviceToHost, s), "copying info");
-  if (hostOverlap)
-    hostOverlap(overlapCtx); // host work of the caller (S1 of the new basis) while the LU runs
-  LU_OK(cudaStreamSynchronize(s), "LU");
-  // Also for a singular nucleus: the interchange of a column without a pivot is the identity and later
-  // ones never touch its position, so hostPerm[info - 1] is the row the first info - 1 pivots parked there.
-  for (int i = 0; i < k; i++)
-    w.hostPerm[i] = i;
-  for (int j = 0; j < k; j++) {
-    int p = w.hostIpiv[j];
-    if (p != j) {
-      int t = w.hostPerm[j];
-      w.hostPerm[j] = w.hostPerm[p];
-      w.hostPerm[p] = t;
-    }
-  }
-  if (info != 0)
-    return info;
-  LU_OK(cudaMemcpyAsync(w.dPerm, w.hostPerm, sizeof(int) * k, cudaMemcpyHostToDevice, s), "copying the permutation");
-  {
-    size_t total = (size_t)ld * k;
-    set_permuted_identity_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(X, k, ld, w.dPerm);
-  }
+  // A^-1 = U^-1 L^-1 P.  Y = U^-1 L^-1 I is computed in X, and X[:, perm[i]] = Y[:, i] is applied by the
+  // transposes at the end.  Column i of L^-1 I is zero above row i, so the forward substitution's outer
+  // step [J0, J1) works on columns < J1 only: k^3 / 3 flops instead of k^3.  Every computed element sees
+  // the operations it saw with all k columns (the skipped ones are exact zeros), and the cuBLAS-or-kernel
+  // choice of each DGEMM is made from the full column count.
+  set_identity_kernel<<<(unsigned)(((size_t)ld * k + 255) / 256), 256, 0, s>>>(X, k, ld);
   // Two-level blocking: triangular solves with the NB x NB diagonal blocks, rank-NB updates only
   // inside an outer block of OB columns, one rank-OB update per outer block for the rest (the bulk
-  // of the 2k^3 flops then runs with K = OB, where the DGEMM is not bound by the C traffic).
+  // of the flops then runs with K = OB, where the DGEMM is not bound by the C traffic).
   constexpr int OB = 128;
-  // Multi-GPU: the columns of X are independent in both substitutions, so rank r computes the block
-  // [xc0, xc1) only (2k^3/W of the 2k^3 flops of this phase) and ONE in-place all-gather of
-  // perC*ld doubles per rank completes X on every rank; the LU above (2/3 k^3) stays replicated.
+  // Multi-GPU: the columns of Y are independent in both substitutions, so rank r computes the block
+  // [xc0, xc1) only and ONE in-place all-gather of perC*ld doubles per rank completes Y on every rank;
+  // the LU above (2/3 k^3) stays replicated.  The forward work of a rank grows with its column index.
   int xc0 = 0, xc1 = k, perC = k;
   if (shardW > 1 && allGather != nullptr) {
     perC = (k + shardW - 1) / shardW;
@@ -766,29 +797,35 @@ int dense_invert(double *A, double *X, int k, int ld, LuWorkspace &w, double sin
   }
   double *const Xr = X + (size_t)xc0 * ld; // this rank's columns, all k rows of them
   const int ncol = xc1 - xc0;
-  // forward: Xr := L^-1 Xr
+  // one thread per column, 32 per CTA: the k columns spread over all SMs
+  auto trsm = [&](int j0, int nb, int n, bool lower) {
+    if (n > 0)
+      trsm_kernel<32><<<(n + 31) / 32, 32, 0, s>>>(A, ld, Xr, ld, j0, nb, 0, n, lower);
+  };
+  // forward: Y := L^-1 Y on columns [xc0, min(xc1, J1))
   for (int J0 = 0; J0 < k; J0 += OB) {
     const int J1 = J0 + OB < k ? J0 + OB : k;
+    const int nf = (xc1 < J1 ? xc1 : J1) - xc0;
+    if (nf <= 0)
+      continue;
     for (int j0 = J0; j0 < J1; j0 += NB) {
       int nb = J1 - j0 < NB ? J1 - j0 : NB;
-      if (ncol > 0)
-        trsm_kernel<<<(ncol + 127) / 128, 128, 0, s>>>(A, ld, Xr, ld, j0, nb, 0, ncol, true);
+      trsm(j0, nb, nf, true);
       int r0 = j0 + nb;
       if (r0 < J1)
-        gemm_sub(Xr + r0, ld, A + (size_t)j0 * ld + r0, ld, Xr + j0, ld, J1 - r0, ncol, nb, s);
+        gemm_sub(Xr + r0, ld, A + (size_t)j0 * ld + r0, ld, Xr + j0, ld, J1 - r0, nf, nb, s, ncol);
     }
     if (J1 < k)
-      gemm_sub(Xr + J1, ld, A + (size_t)J0 * ld + J1, ld, Xr + J0, ld, k - J1, ncol, J1 - J0, s);
+      gemm_sub(Xr + J1, ld, A + (size_t)J0 * ld + J1, ld, Xr + J0, ld, k - J1, nf, J1 - J0, s, ncol);
   }
-  // backward: Xr := U^-1 Xr
+  // backward: Y := U^-1 Y
   const int lastOuter = ((k - 1) / OB) * OB;
   for (int J0 = lastOuter; J0 >= 0; J0 -= OB) {
     const int J1 = J0 + OB < k ? J0 + OB : k;
     const int lastInner = J0 + ((J1 - J0 - 1) / NB) * NB;
     for (int j0 = lastInner; j0 >= J0; j0 -= NB) {
       int nb = J1 - j0 < NB ? J1 - j0 : NB;
-      if (ncol > 0)
-        trsm_kernel<<<(ncol + 127) / 128, 128, 0, s>>>(A, ld, Xr, ld, j0, nb, 0, ncol, false);
+      trsm(j0, nb, ncol, false);
       if (j0 > J0)
         gemm_sub(Xr + J0, ld, A + (size_t)j0 * ld + J0, ld, Xr + j0, ld, j0 - J0, ncol, nb, s);
     }
@@ -800,9 +837,20 @@ int dense_invert(double *A, double *X, int k, int ld, LuWorkspace &w, double sin
     if (allGather(comm, X, sizeof(double) * (size_t)perC * ld, s) != 0)
       return -98;
   }
-  zero_padding_kernel<<<(k + 255) / 256, 256, 0, s>>>(X, k, ld);
-  LU_OK(cudaGetLastError(), "zero_padding_kernel launch");
-  return 0;
+  // A := X^T (the LU factors are dead): row perm[i] of A is column i of Y, read from column invPerm[r]
+  // for row r; then X := A^T
+  invert_perm_kernel<<<(k + 255) / 256, 256, 0, s>>>(w.dPerm, w.dInvPerm, k);
+  launch_transpose(X, A, k, ld, w.dInvPerm, s);
+  launch_transpose(A, X, k, ld, nullptr, s);
+  LU_OK(cudaGetLastError(), "transpose launches");
+  if (hostOverlap)
+    hostOverlap(overlapCtx); // host work of the caller (S1 of the new basis) while the GPU works
+  // pageable destinations: these copies wait for the stream, so they come after all launches
+  LU_OK(cudaMemcpyAsync(w.hostPerm, w.dPerm, sizeof(int) * k, cudaMemcpyDeviceToHost, s), "copying the permutation");
+  int info = 0;
+  LU_OK(cudaMemcpyAsync(&info, w.dInfo, sizeof(int), cudaMemcpyDeviceToHost, s), "copying info");
+  LU_OK(cudaStreamSynchronize(s), "dense_invert");
+  return info;
 }
 
 } // namespace clpb
