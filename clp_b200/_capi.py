@@ -50,6 +50,10 @@ SIGNATURES = {
     "Clpb_lastSolveWasHot": (ctypes.c_int, [ctypes.c_void_p]),
     "Clpb_refactorizationInterval": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int]),
     "Clpb_dual": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int]),
+    "Clpb_dualRanging": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, c_int_p, c_double_p, c_int_p, c_double_p,
+                                        c_int_p, c_double_p, c_double_p]),
+    "Clpb_primalRanging": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, c_int_p, c_double_p, c_int_p, c_double_p,
+                                          c_int_p]),
     "Clpb_status": (ctypes.c_int, [ctypes.c_void_p]),
     "Clpb_objectiveValue": (ctypes.c_double, [ctypes.c_void_p]),
     "Clpb_numberIterations": (ctypes.c_int, [ctypes.c_void_p]),

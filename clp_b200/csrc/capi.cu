@@ -267,6 +267,23 @@ int Clpb_dual(Clpb_Simplex *model, int)
 {
   return guarded([&] { return model->e.dual(); });
 }
+int Clpb_dualRanging(Clpb_Simplex *model, int numberCheck, const int *which, double *costIncrease,
+                     int *sequenceIncrease, double *costDecrease, int *sequenceDecrease,
+                     double *valueIncrease, double *valueDecrease)
+{
+  return guarded([&] {
+    return model->e.dualRanging(numberCheck, which, costIncrease, sequenceIncrease, costDecrease, sequenceDecrease,
+                                valueIncrease, valueDecrease);
+  });
+}
+int Clpb_primalRanging(Clpb_Simplex *model, int numberCheck, const int *which, double *valueIncrease,
+                       int *sequenceIncrease, double *valueDecrease, int *sequenceDecrease)
+{
+  return guarded([&] {
+    return model->e.primalRanging(numberCheck, which, valueIncrease, sequenceIncrease, valueDecrease,
+                                  sequenceDecrease);
+  });
+}
 int Clpb_status(Clpb_Simplex *model) { return model->e.problemStatus; }
 double Clpb_objectiveValue(Clpb_Simplex *model) { return model->e.objectiveValue; }
 int Clpb_numberIterations(Clpb_Simplex *model) { return model->e.numberIterations; }

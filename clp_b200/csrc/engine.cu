@@ -63,6 +63,8 @@ void Engine::freeAll()
   stream = nullptr;
   deviceReady = false;
   factorsValid = false;
+  optimalOnDevice = false;
+  rw = RangeWork{};
   nucCap = 0;
   s1Cap = 0;
 }
@@ -111,6 +113,7 @@ int Engine::loadProblem(int numberColumns, int numberRows, const int *columnStar
     hUpper[n + i] = rowUpper ? up(rowUpper[i]) : kInf;
   }
   haveUserStatus = false;
+  optimalOnDevice = false;
   hStatus.assign(nm, atLowerBound);
   for (int i = 0; i < m; i++)
     hStatus[n + i] = basic;
@@ -138,6 +141,7 @@ void Engine::setStatus(const unsigned char *st)
   hStatus.assign(st, st + nm);
   haveUserStatus = true;
   factorsValid = false; // a basis handed in from outside is factorized afresh
+  optimalOnDevice = false;
 }
 
 void Engine::buildRowCopy(const std::vector<double> &val, std::vector<int> &rowStart,
@@ -280,13 +284,18 @@ int Engine::cycleFor(int k) const
   return cycle;
 }
 
+// what the device copy was built for: a later scaling() / factorizationFrequency / timing change
+// rebuilds it instead of being silently ignored (and leaves no optimal basis to range)
+long long Engine::deviceSignature() const
+{
+  return (long long)scalingFlag * 1000003ll + (long long)factorizationFrequency * 101ll + (timing ? 7 : 0) +
+         (long long)worldSize * 13ll + (long long)rank * 17ll + (shardActive() ? 31 : 0) +
+         (long long)(shardPanelMode + 1) * 37ll + (long long)dualRowPivot * 41ll;
+}
+
 int Engine::setupDevice()
 {
-  // what the device copy was built for: a later scaling() / factorizationFrequency / timing change
-  // rebuilds it instead of being silently ignored
-  const long long signature = (long long)scalingFlag * 1000003ll + (long long)factorizationFrequency * 101ll +
-                              (timing ? 7 : 0) + (long long)worldSize * 13ll + (long long)rank * 17ll +
-                              (shardActive() ? 31 : 0) + (long long)(shardPanelMode + 1) * 37ll + (long long)dualRowPivot * 41ll;
+  const long long signature = deviceSignature();
   if (deviceReady && signature == readySignature)
     return 0;
   if (deviceReady)
@@ -422,6 +431,16 @@ int Engine::setupDevice()
   dZ = dalloc<double>(n);
   dObj = dalloc<double>(2);
   dCounters = dalloc<int>(4);
+  rw.rho = dalloc<double>((size_t)m * kRangeBatch);
+  rw.y = dalloc<double>((size_t)kRangeBatch * roundUp(m, 8));
+  rw.x = dalloc<double>((size_t)kRangeBatch * m);
+  rw.seq = dalloc<int>(kRangeBatch);
+  rw.other = dalloc<int>(kRangeBatch);
+  rw.partRatio = dalloc<double>((size_t)2 * kRangeBatch * kRangeBlocks);
+  rw.partSeq = dalloc<int>((size_t)2 * kRangeBatch * kRangeBlocks);
+  rw.outRatio = dalloc<double>(2 * kRangeBatch);
+  rw.outSeq = dalloc<int>(2 * kRangeBatch);
+  rw.alphaOther = dalloc<double>(kRangeBatch);
   CUDA_OK(lu_workspace_reserve(lu, m));
   CUDA_OK(cudaMallocHost(&hState, sizeof(IterState)));
   CUDA_OK(cudaMallocHost(&hRec, sizeof(IterRecord) * d.recCap));
@@ -1106,6 +1125,7 @@ void Engine::chgBounds(const double *columnLower, const double *columnUpper, con
   }
   if (deviceReady)
     boundsToWorking(); // the scale factors of the device copy stay in force
+  optimalOnDevice = false;
 }
 
 // Re-impose the bounds on the device-resident state of the previous solve and recompute x_B through the
@@ -1129,6 +1149,7 @@ int Engine::hotPrepare()
 
 int Engine::startup()
 {
+  optimalOnDevice = false;
   setupDevice();
   resetStateForRun();
   largestPerturbation = 0.0;
@@ -1158,6 +1179,7 @@ int Engine::dual()
   numberRefactorizations = 0;
   kernelLaunches = 0;
   phase = PhaseTimes();
+  optimalOnDevice = false;
   if (m == 0 || n == 0)
     return trivialSolve();
   driftMeasured = false;
@@ -1408,6 +1430,8 @@ int Engine::dual()
   cudaEventDestroy(evStart);
   cudaEventDestroy(evStop);
   downloadSolution();
+  // status 0 is only reached on fresh factors (STOP_NO_ROW with numEtas == 0): ranging can use them
+  optimalOnDevice = problemStatus == 0;
   secondsInLoop = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
   return problemStatus;
 }
@@ -1416,6 +1440,7 @@ int Engine::dual()
 // plug-in level entry points (host buffers in, host buffers out)
 int Engine::factorize(const int *basicSequence, int *pivotVariableOut)
 {
+  optimalOnDevice = false;
   setupDevice();
   hStatus.assign(nm, atLowerBound);
   for (int p = 0; p < m; p++)
@@ -1451,6 +1476,7 @@ int Engine::updateColumnTranspose(double *vec)
 
 int Engine::replaceColumn(int sequenceIn, int pivotRow)
 {
+  optimalOnDevice = false;
   fetchState();
   if (hState->numEtas >= std::min(currentCycle, d.tmax))
     return 5; // maximum pivots reached (ClpFactorization.hpp:87)
@@ -1490,6 +1516,7 @@ void Engine::times(double scalar, const double *x, double *y)
 int Engine::dualColumnTest(const double *alphaRow, const double *dj, const unsigned char *stat,
                            int sigma, double infeas, double *theta)
 {
+  optimalOnDevice = false;
   setupDevice();
   resetStateForRun();
   CUDA_OK(cudaMemcpy(d.alphaRow, alphaRow, sizeof(double) * nm, cudaMemcpyHostToDevice));
@@ -1524,6 +1551,7 @@ int Engine::dualColumnTest(const double *alphaRow, const double *dj, const unsig
 
 int Engine::iterate(int count)
 {
+  optimalOnDevice = false;
   int total = 0;
   while (count > 0) {
     int c = std::min(count, d.recCap);
@@ -1554,6 +1582,7 @@ int Engine::iterate(int count)
 //                       append) + ClpSimplex::housekeeping (src/ClpSimplex.cpp:2065)
 int Engine::pivotRowStep(int *sequenceOut, int *direction, double *infeasibility)
 {
+  optimalOnDevice = false;
   CUDA_OK(cudaMemsetAsync(&d.st->stop, 0, sizeof(int), stream));
   launch_chuzr(d, stream);
   kernelLaunches += 2;
@@ -1592,6 +1621,7 @@ int Engine::btranPriceStep(double *rho, double *alphaRow)
 
 int Engine::dualColumnStep(double *theta, double *alpha)
 {
+  optimalOnDevice = false;
   if (!launch_row_pass(d, stream))
     throw std::runtime_error("row pass launch failed");
   kernelLaunches += 1;
@@ -1609,6 +1639,7 @@ int Engine::dualColumnStep(double *theta, double *alpha)
 
 double Engine::updateWeightsStep(int *returnCode)
 {
+  optimalOnDevice = false;
   launch_ftran_iteration(d, stream);
   kernelLaunches += 4;
   fetchState();
@@ -1624,6 +1655,7 @@ double Engine::updateWeightsStep(int *returnCode)
 
 int Engine::updatePrimalStep(double *changeInObjective)
 {
+  optimalOnDevice = false;
   fetchState();
   const int r = hState->pivotRow, q = hState->seqIn;
   const double gain = hState->thetaDual * hState->infeas; // dual objective gain of the step
@@ -1709,6 +1741,7 @@ int Engine::updateColumnFT(double *vec)
 // update buffers, 5 the maximum number of pivots (factorizationFrequency) is reached.
 int Engine::replaceColumnChecked(int sequenceIn, int pivotRow, double pivotCheck, double acceptable)
 {
+  optimalOnDevice = false;
   fetchState();
   const int t = hState->numEtas;
   if (t >= std::min(currentCycle, d.tmax))

@@ -250,5 +250,27 @@ int dense_invert(double *A, double *X, int k, int ld, LuWorkspace &w, double sin
                  cudaStream_t s, int shardW = 1, int shardRank = 0,
                  int (*allGather)(void *, void *, size_t, void *) = nullptr, void *comm = nullptr,
                  void (*hostOverlap)(void *) = nullptr, void *overlapCtx = nullptr);
+// ranging.cu -- batched sensitivity analysis on fresh factors (DESIGN.md "Ranging").  One pass handles up
+// to kRangeBatch right-hand sides; the scratch is allocated with the other device buffers.
+constexpr int kRangeBatch = 16;
+constexpr int kRangeBlocks = 1024; // most CTAs of a ranging pass = partial-result slots per right-hand side
+struct RangeWork {
+  double *rho;        // [m][kRangeBatch] rows of B^-1 (row-major: one row index = one 128-byte line)
+  double *y;          // [kRangeBatch][roundUp(m, 8)] nucleus part of the FTRAN'd columns
+  double *x;          // [kRangeBatch][m] FTRAN'd columns by position
+  int *seq;           // [kRangeBatch] dual: position of the basic variable; primal: entering sequence
+  int *other;         // [kRangeBatch] primal: sequence excluded from the ratio test (-1: none)
+  double *partRatio;  // [2][kRangeBatch][kRangeBlocks] per-CTA best (ratio, sequence), up then down
+  int *partSeq;
+  double *outRatio;   // [2][kRangeBatch] final best ratio per direction (+1e31 / +1e30 when none)
+  int *outSeq;        // [2][kRangeBatch] its sequence, -1 when none
+  double *alphaOther; // [kRangeBatch] FTRAN'd entry at the excluded sequence's position (0 when absent)
+};
+// Dual ratio test of the tableau rows of the nb basic variables at positions w.seq[0..nb):
+// checkDualRatios (ClpSimplexOther.cpp:266-374) with the smallest ratio winning, ties to the smallest sequence.
+void launch_range_dual(const DeviceModel &d, const RangeWork &w, int nb, double dualTolerance, cudaStream_t s);
+// Primal ratio test of the FTRAN'd columns of the nb sequences w.seq[0..nb), both directions:
+// checkPrimalRatios (ClpSimplexOther.cpp:958-1001), the position of w.other[b] left out.
+void launch_range_primal(const DeviceModel &d, const RangeWork &w, int nb, cudaStream_t s);
 
 } // namespace clpb

@@ -137,6 +137,14 @@ public:
   void getDeviceVector(const char *name, double *out);
   int startup();                            // status -> basis, factorize, compute primals/duals
 
+  // ---- sensitivity analysis on the optimal basis the last dual() left on the device
+  // (ClpSimplex::dualRanging / primalRanging, src/ClpSimplex.hpp:437,455 -> ClpSimplexOther.cpp:50,770;
+  // ranging.cu).  0 ranges written; 1 no optimal basis resident (nothing written); -1 a which[i] >= n+m.
+  int dualRanging(int numberCheck, const int *which, double *costIncrease, int *sequenceIncrease,
+                  double *costDecrease, int *sequenceDecrease, double *valueIncrease, double *valueDecrease);
+  int primalRanging(int numberCheck, const int *which, double *valueIncrease, int *sequenceIncrease,
+                    double *valueDecrease, int *sequenceDecrease);
+
   int numberRows() const { return m; }
   int numberColumns() const { return n; }
   long long numberElements() const { return (long long)hColStart.empty() ? 0 : hColStart[n]; }
@@ -156,6 +164,14 @@ private:
   cudaStream_t stream = nullptr;
   bool deviceReady = false;
   bool factorsValid = false; // a factorization of the current device basis exists
+  // the last dual() ended with status 0 on the device (fresh factors, working sol / dj / status); every
+  // change of the problem, its bounds, the status or the device state clears it
+  bool optimalOnDevice = false;
+  long long deviceSignature() const; // what setupDevice built the device copy for
+  RangeWork rw{};                    // ranging scratch (ranging.cu), allocated by setupDevice
+  struct RangeSnapshot;
+  int rangingSnapshot(RangeSnapshot &r);
+  void rangePass(bool dual, const int *seqs, const int *others, int nb, double *ratio, int *seq, double *alphaOther);
   void boundsToWorking();    // hLower/hUpper -> wLower/wUpper with the scale factors in force
   int hotPrepare();
   long long readySignature = -1;

@@ -205,6 +205,45 @@ class ClpSimplex:
             raise RuntimeError("clp_b200: CUDA failure inside dual()")
         return rc
 
+    # ---- ClpSimplex::dualRanging / primalRanging (sensitivity analysis of the optimal basis) ----
+    def _which(self, which):
+        if which is None:
+            return np.arange(self.numberColumns() + self.numberRows(), dtype=np.int32)
+        return np.ascontiguousarray(which, dtype=np.int32)
+
+    def _ranging_rc(self, rc):
+        self._chk(rc)
+        if rc == 1:
+            raise RuntimeError("clp_b200: no optimal basis on the device (solve with dual() first)")
+        if rc == -1:
+            raise ValueError("ranging: a sequence is outside 0 .. n+m-1")
+
+    def dualRanging(self, which=None, values=False):
+        """ClpSimplex::dualRanging on the basis of the last optimal dual().  which: sequences (columns
+        0..n-1, rows n..n+m-1; None = all).  Returns (costIncrease, sequenceIncrease, costDecrease,
+        sequenceDecrease), plus (valueIncrease, valueDecrease) when values is true."""
+        w = self._which(which)
+        k = len(w)
+        ci, cd = np.zeros(k), np.zeros(k)
+        si, sd = np.full(k, -1, np.int32), np.full(k, -1, np.int32)
+        vi = vd = None
+        if values:
+            vi, vd = np.zeros(k), np.zeros(k)
+        self._ranging_rc(self._L.Clpb_dualRanging(self._h, k, _ip(w), _dp(ci), _ip(si), _dp(cd), _ip(sd),
+                                                  _dp(vi) if values else None, _dp(vd) if values else None))
+        return (ci, si, cd, sd, vi, vd) if values else (ci, si, cd, sd)
+
+    def primalRanging(self, which=None):
+        """ClpSimplex::primalRanging on the basis of the last optimal dual().  Returns (valueIncrease,
+        sequenceIncrease, valueDecrease, sequenceDecrease); for basic, free and superbasic variables the
+        reference's assignment is kept: valueDecrease = max(0, upper - x), valueIncrease = max(0, x - lower)."""
+        w = self._which(which)
+        k = len(w)
+        vi, vd = np.zeros(k), np.zeros(k)
+        si, sd = np.full(k, -1, np.int32), np.full(k, -1, np.int32)
+        self._ranging_rc(self._L.Clpb_primalRanging(self._h, k, _ip(w), _dp(vi), _ip(si), _dp(vd), _ip(sd)))
+        return vi, si, vd, sd
+
     def status(self): return self._L.Clpb_status(self._h)
     def isProvenOptimal(self): return self.status() == 0
     def isProvenPrimalInfeasible(self): return self.status() == 1

@@ -122,6 +122,30 @@ void Clpb_primalRowSolution(Clpb_Simplex *model, double *rowActivity /* m */);
 void Clpb_dualColumnSolution(Clpb_Simplex *model, double *reducedCost /* n */);
 void Clpb_dualRowSolution(Clpb_Simplex *model, double *rowPrice /* m */);
 void Clpb_statusArray(Clpb_Simplex *model, unsigned char *status /* n+m */);
+/* Sensitivity analysis on the optimal basis the last Clpb_dual left on the device.
+   ClpSimplex::dualRanging (src/ClpSimplex.hpp:437 -> ClpSimplexOther.cpp:50-260, checkDualRatios :266-374):
+   for each which[i] (0..n-1 columns, n..n+m-1 rows) how far its cost can rise / fall before the basis
+   changes, and the sequence that would enter.  A basic variable gets the ratio test of its tableau row,
+   the smallest ratio winning and ties going to the smallest sequence; a nonbasic one at a bound gets
+   max(0, -+dj) and itself; fixed variables stay unbounded; free / superbasic ones get 0 and themselves.
+   which[i] < 0 gives 0 / -1 / 0 / -1.  valueIncrease / valueDecrease may be NULL; otherwise they get the
+   value of which[i] once the reported sequence has entered (primalRanging1, :848-953), the current value
+   when that sequence is free or superbasic.
+   ClpSimplex::primalRanging (:455 -> ClpSimplexOther.cpp:770-846, checkPrimalRatios :958-1001): for each
+   nonbasic or fixed which[i], how far its value can move up / down before a basic variable reaches a bound
+   (the variable's own other bound is ignored) and that basic variable's sequence.  For basic, free and
+   superbasic variables the reference's assignment is kept as it stands: valueDecrease = max(0, upper - x),
+   valueIncrease = max(0, x - lower).
+   Unbounded sides are DBL_MAX with sequence -1; results are in the caller's units (scaled solves are
+   unscaled with :215-227 and :824-840).  The engine only minimizes.  Both return 0, 1 when no optimal basis
+   is resident (never solved, the last Clpb_dual did not return 0 or needed no device, or the problem,
+   bounds, status or device parameters changed since, or the model is sharded; nothing is written), -1 when
+   some which[i] >= n+m (for primal ranging also < 0), CLPB_NO_DEVICE / -99 as elsewhere. */
+int Clpb_dualRanging(Clpb_Simplex *model, int numberCheck, const int *which, double *costIncrease,
+                     int *sequenceIncrease, double *costDecrease, int *sequenceDecrease,
+                     double *valueIncrease, double *valueDecrease);
+int Clpb_primalRanging(Clpb_Simplex *model, int numberCheck, const int *which, double *valueIncrease,
+                       int *sequenceIncrease, double *valueDecrease, int *sequenceDecrease);
 /* measurement: seconds in the iteration loop, kernels launched, per-phase device ms
    (order: chuzr, btran, price, chuzc, dualUpdate, ftran, update, refactor, samples, then the
    single kernels priceKernel, ftranGemv, btranGemv, then the algorithmic bytes summed over the
