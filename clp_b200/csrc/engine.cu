@@ -1787,6 +1787,14 @@ void Engine::getDeviceVector(const char *name, double *out)
     CUDA_OK(cudaMemcpy(out, d.rho, sizeof(double) * m, cudaMemcpyDeviceToHost));
   else if (s == "alphaRow")
     CUDA_OK(cudaMemcpy(out, d.alphaRow, sizeof(double) * nm, cudaMemcpyDeviceToHost));
+  else if (s == "rhs3")
+    CUDA_OK(cudaMemcpy(out, d.rhs3, sizeof(double) * 3 * (size_t)m, cudaMemcpyDeviceToHost));
+  else if (s == "lower")
+    CUDA_OK(cudaMemcpy(out, d.lower, sizeof(double) * nm, cudaMemcpyDeviceToHost));
+  else if (s == "upper")
+    CUDA_OK(cudaMemcpy(out, d.upper, sizeof(double) * nm, cudaMemcpyDeviceToHost));
+  else if (s == "cost")
+    CUDA_OK(cudaMemcpy(out, d.cost, sizeof(double) * nm, cudaMemcpyDeviceToHost));
   else if (s == "pivotVariable") {
     std::vector<int> pv(m);
     CUDA_OK(cudaMemcpy(pv.data(), d.pivotVariable, sizeof(int) * m, cudaMemcpyDeviceToHost));

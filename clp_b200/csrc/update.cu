@@ -426,21 +426,22 @@ __global__ void unpack_column_kernel(DeviceModel d, int seq, double *__restrict_
       out[i] = (i == seq - d.n) ? -1.0 : 0.0;
     return;
   }
-  // zero fill then scatter by the first block (columns are short)
+  // zero fill; unpack_scatter_kernel then writes the entries
   if (i < d.m)
     out[i] = 0.0;
 }
+// grid-stride over the entries: a column may hold up to m entries
 __global__ void unpack_scatter_kernel(DeviceModel d, int seq, double *__restrict__ out)
 {
-  int e = d.colStart[seq] + blockIdx.x * blockDim.x + threadIdx.x;
-  if (e < d.colStart[seq + 1])
+  const int e1 = d.colStart[seq + 1];
+  for (int e = d.colStart[seq] + blockIdx.x * blockDim.x + threadIdx.x; e < e1; e += gridDim.x * blockDim.x)
     out[d.rowIdx[e]] = d.val[e];
 }
 void launch_unpack_column(const DeviceModel &d, int seq, double *out, cudaStream_t s)
 {
   unpack_column_kernel<<<(d.m + 255) / 256, 256, 0, s>>>(d, seq, out);
   if (seq < d.n)
-    unpack_scatter_kernel<<<64, 256, 0, s>>>(d, seq, out); // columns up to 16384 entries
+    unpack_scatter_kernel<<<64, 256, 0, s>>>(d, seq, out);
 }
 
 // Product-form update outside the simplex loop (replaceColumn entry point / parity tests):

@@ -420,7 +420,7 @@ class ClpSimplex:
     def deviceVector(self, name):
         n, m = self.numberColumns(), self.numberRows()
         size = {"sol": n + m, "dj": n + m, "rho": m, "alphaRow": n + m, "pivotVariable": m,
-                "status": n + m}[name]
+                "status": n + m, "rhs3": 3 * m, "lower": n + m, "upper": n + m, "cost": n + m}[name]
         out = np.zeros(size)
         self._L.Clpb_getDeviceVector(self._h, name.encode(), _dp(out))
         return out

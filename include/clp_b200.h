@@ -247,7 +247,10 @@ int Clpb_startup(Clpb_Simplex *model);
 int Clpb_iterate(Clpb_Simplex *model, int count);
 void Clpb_getWeights(Clpb_Simplex *model, double *weights /* m */);
 /* debug reads of device vectors: "sol","dj" (n+m), "rho" (m), "alphaRow" (n+m),
-   "pivotVariable" (m, as doubles), "status" (n+m, as doubles) */
+   "pivotVariable" (m, as doubles), "status" (n+m, as doubles), the working bounds and costs
+   "lower","upper","cost" (n+m), and "rhs3" (3 x m): after Clpb_dualColumn / Clpb_dualColumnDevice
+   the row pass's FTRAN right-hand sides [a_q, rho, flip column], after Clpb_updateWeights their
+   FTRAN results [B^-1 a_q, B^-1 rho, B^-1 flip column] */
 void Clpb_getDeviceVector(Clpb_Simplex *model, const char *name, double *out);
 
 #ifdef __cplusplus

@@ -49,12 +49,25 @@ def test_stepwise_plugin_calls_take_the_pivots_of_the_fused_iteration():
     np.testing.assert_array_equal(a.weights(), b.weights())
 
 
-@pytest.mark.parametrize("shape", [(400, 6000, 0.02, 3), (1200, 9000, 0.01, 4)])
+def _price_variant(m):
+    """the price_ldg_kernel instance launch_price (price.cu) selects: rho in shared memory with two 640-thread
+    CTAs per SM (<= 112 KiB), with one 1024-thread CTA (<= 224 KiB), or read through L1/L2"""
+    b = 8 * m
+    return "640x2,smem" if b <= 112 * 1024 else "1024x1,smem" if b <= 224 * 1024 else "640x2,ldg"
+
+
+@pytest.mark.parametrize("shape", [(400, 6000, 0.02, 3, "640x2,smem"), (1200, 9000, 0.01, 4, "640x2,smem"),
+                                   (14337, 4000, 0.01, 5, "1024x1,smem"), (28673, 4000, 0.01, 6, "640x2,ldg"),
+                                   (40000, 4000, 0.01, 7, "640x2,ldg")])
 def test_price_kernel_row_against_oracle(shape):
     """the tableau row the HOT price kernel (price_ldg_kernel) writes for the BTRAN'd rho, dense and
-    sparse rho: alphaRow_j = rho^T a_j for every nonbasic column (1e-12, DESIGN.md section 6)"""
-    m, n, dens, seed = shape
+    sparse rho: alphaRow_j = rho^T a_j for every nonbasic column (1e-12, DESIGN.md section 6).  The three
+    launch variants, and (m >= 14 337 at 1 % density) columns longer than the 128 entries of the first pass"""
+    m, n, dens, seed, variant = shape
+    assert _price_variant(m) == variant
     lp = G.random_sparse_lp(m, n, dens, seed)
+    if m > 10000:
+        assert np.diff(lp.col_start).mean() > 128
     A = lp.to_scipy()
     s = engine(lp, factorizationFrequency=400)
     assert s.startup() == 0
@@ -93,21 +106,36 @@ def _row_case(rng, nm, kind):
         dj[:25] = 0.0
     elif kind == "wide":          # ratios spread over many octaves: the Harris bound leaves the listed window
         dj *= np.exp(rng.uniform(-20, 5, size=nm))
+    elif kind == "flip-wide":     # thousands of passed break points with ranges over 12 decades: the flips and
+        rangeb = 10.0 ** rng.uniform(-6, 6, size=nm)   # the fixed-point flip column (DESIGN.md section 4)
+        alpha = np.where(alpha != 0.0, np.sign(alpha) * rng.uniform(0.5, 1.0, size=nm) / rangeb, 0.0)
+        dj = rng.uniform(0.0, 1.0, size=nm) * np.abs(alpha)   # ratios U(0, 1), independent of the range;
+        dj[nm - 64:] *= 1e-3                                   # the slacks' come first: slack flips too
     dj = np.where(stat == 2, -dj, dj)
     return alpha, dj, rangeb, stat
 
 
-@pytest.mark.parametrize("kind", ["plain", "ties", "boxed-small", "free", "wide"])
-@pytest.mark.parametrize("n", [20000, 400000])   # 1 and 4 entries per thread of the cooperative kernel
-def test_dual_column_on_adversarial_rows_against_reference_rule(kind, n):
+@pytest.mark.parametrize("kind", ["plain", "ties", "boxed-small", "free", "wide", "flip-wide"])
+@pytest.mark.parametrize("n", [20000, 400000, "E2", "E8"])   # 1 and 4 entries per thread of the cooperative kernel;
+def test_dual_column_on_adversarial_rows_against_reference_rule(kind, n):   # 2 and 8 on this card
     """Clpb_dualColumn, i.e. the cooperative row_pass_kernel of the fused iteration, on adversarial rows, against
     the oracle's restatement of the reference's SORTED-PASS dualColumn (ClpSimplexDual.cpp:4331-4658):
     never beyond its break point and within the histogram resolution + Harris slack of it; and identical
-    to the bucketed restatement."""
+    to the bucketed restatement.  The dual update, the bound flips and the flip column the same kernel
+    writes against tests/iteration_ref.py."""
     import zlib
 
-    rng = np.random.default_rng(zlib.crc32(f"{kind}-{n}".encode()))
+    import torch
+
+    import iteration_ref as R
+
     m = 64
+    if isinstance(n, str):  # n+m in the row_pass_kernel<2> / <8> range of this card
+        S = torch.cuda.get_device_properties(0).multi_processor_count * 1024
+        E = int(n[1:])
+        n = int((E - 0.5) * S) - m
+        assert -(-(n + m) // S) == E
+    rng = np.random.default_rng(zlib.crc32(f"{kind}-{n}".encode()))
     nm = n + m
     alpha, dj, rangeb, stat = _row_case(rng, nm, kind)
     # a model that only provides sizes and bounds 0 <= x <= range (one entry per column)
@@ -118,7 +146,9 @@ def test_dual_column_on_adversarial_rows_against_reference_rule(kind, n):
     lp = G.LP("rowpass", m, n, start, rows, np.ones(n), np.where(stat[:n] == 0, -1e30, 0.0), ub[:n].copy(),
               np.zeros(n), np.zeros(m), ub[n:].copy())
     s = engine(lp)
-    infeas, sigma = 3.0, 1
+    # flip-wide: every candidate uses up |alpha| * range ~ 1 of the slope, so thousands pass before 3 000 is
+    # used up, and |alpha| (theta - ratio) exceeds the dual tolerance up to ranges of 1e6
+    infeas, sigma = (3.0e3 if kind == "flip-wide" else 3.0), 1
     q, theta = s.dualColumn(alpha, dj, stat, sigma, infeas)
     idx = np.nonzero((alpha != 0) & (np.abs(alpha) > 1e-12))[0]
     rng_arg = np.where(stat == 0, 1e30, rangeb)
@@ -132,9 +162,11 @@ def test_dual_column_on_adversarial_rows_against_reference_rule(kind, n):
     assert theta == theta_b
     slack = 2e-6 / max(1e-7, abs(alpha[q]))
     assert theta >= theta_c * (1 - 1e-3) - slack
-    if kind != "boxed-small":
+    if kind not in ("boxed-small", "flip-wide"):
         assert theta <= theta_c * (1 + 1e-9) + slack
-    else:
+    elif kind == "boxed-small":
+        # (flip-wide passes thousands of break points too; there the bucketed restatement itself passes up to
+        # ~1e-4 relative more slope than the infeasibility, so only its identity with the kernel is checked)
         # the reference gives up after MAXTRY = 100 passes (ClpSimplexDual.cpp:4400) and stops short of the
         # point where the slope is used up; the histogram rule has no pass limit.  What must hold is that
         # the step is still a valid long step: the break points passed do not overshoot the infeasibility
@@ -146,6 +178,23 @@ def test_dual_column_on_adversarial_rows_against_reference_rule(kind, n):
     ab = sigma * alpha[q]
     assert (stat[q] == 3 and ab > 0) or (stat[q] == 2 and ab < 0) or stat[q] == 0
     assert abs(alpha[q]) >= 1e-7
+    # the dual update, the bound flips and the flip column (rhs3[2m:]) the same kernel wrote
+    lower, upper = s.deviceVector("lower"), s.deviceVector("upper")
+    fin = R.finalize_row(alpha[:n], -alpha[n:], stat, n)
+    np.testing.assert_array_equal(s.deviceVector("alphaRow"), fin)
+    du = R.dual_update(fin, dj, stat, lower, upper, np.zeros(nm), np.zeros(nm), sigma, theta, q)
+    status1, dj1, sol1 = s.deviceVector("status").astype(np.uint8), s.deviceVector("dj"), s.deviceVector("sol")
+    keep = np.ones(nm, dtype=bool)
+    keep[du["edge"]] = False
+    assert np.all(np.abs(dj1 - du["dj"])[keep] <= du["dj_bound"][keep])
+    flips = np.flatnonzero(status1 != stat)
+    assert set(flips.tolist()) ^ set(du["flips"].tolist()) <= set(du["edge"].tolist())
+    np.testing.assert_array_equal(status1[keep], du["status"][keep])
+    np.testing.assert_array_equal(sol1[flips], np.where(status1[flips] == R.AT_UPPER, upper[flips], lower[flips]))
+    fl, fl_bound = R.flip_column(R.ext_matrix(lp), flips, status1, lower, upper, 1.0)
+    assert np.all(np.abs(s.deviceVector("rhs3")[2 * m:] - fl) <= fl_bound)
+    if kind == "flip-wide":
+        assert len(flips) >= 1000 and (flips >= n).any()
 
 
 def test_packed_forms_match_dense():
