@@ -95,6 +95,7 @@ SIGNATURES = {
                                                  c_int_p, c_int_p, c_double_p]),
     "Clpb_startup": (ctypes.c_int, [ctypes.c_void_p]),
     "Clpb_iterate": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int]),
+    "Clpb_refresh": (ctypes.c_int, [ctypes.c_void_p]),
     "Clpb_getWeights": (None, [ctypes.c_void_p, c_double_p]),
     "Clpb_getDeviceVector": (None, [ctypes.c_void_p, ctypes.c_char_p, c_double_p]),
 }

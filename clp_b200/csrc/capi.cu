@@ -557,6 +557,10 @@ int Clpb_iterate(Clpb_Simplex *model, int count)
 {
   return guarded([&] { return model->e.iterate(count); });
 }
+int Clpb_refresh(Clpb_Simplex *model)
+{
+  return guarded([&] { return model->e.refresh(); });
+}
 void Clpb_getWeights(Clpb_Simplex *model, double *weights)
 {
   guarded([&] {

@@ -784,10 +784,12 @@ int Engine::refactor()
       fprintf(stderr, "clp_b200: singular basis: structural %d out, slack of row %d in\n",
               seqLeave, rowEnter);
     // new basis list (positions are re-canonicalised on the next attempt)
+    int posLeave = -1;
     for (int p = 0; p < m; p++)
-      if (newPivot[p] == seqLeave)
+      if (newPivot[p] == seqLeave) {
         newPivot[p] = n + rowEnter;
-    // make srcPos consistent: treat as a fresh basis for weights of the new slack
+        posLeave = p;
+      }
     hPivot = newPivot;
     hStatus[n + rowEnter] = basic;
     double lo = wLower[seqLeave], up = wUpper[seqLeave];
@@ -808,7 +810,10 @@ int Engine::refactor()
     unsigned char bs = basic;
     CUDA_OK(cudaMemcpy(d.status + n + rowEnter, &bs, 1, cudaMemcpyHostToDevice));
     CUDA_OK(cudaMemcpy(d.sol + seqLeave, &x, sizeof(double), cudaMemcpyHostToDevice));
-    // weights: permute to the (old->new) order first so the next attempt starts from newPivot
+    // weights: permute to the (old->new) order first so the next attempt starts from newPivot; the slack
+    // that came in starts at 1 like any variable new to the basis (ClpDualRowSteepest::saveWeights mode 2,
+    // src/ClpDualRowSteepest.cpp:773ff), not at the weight of the structural it replaces
+    srcPos[posLeave] = -1;
     CUDA_OK(cudaMemcpy(dSrcPos, srcPos.data(), sizeof(int) * m, cudaMemcpyHostToDevice));
     launch_permute_weights(d.weights, dWeightsTmp, dSrcPos, m, stream);
     CUDA_OK(cudaMemcpyAsync(d.weights, dWeightsTmp, sizeof(double) * m, cudaMemcpyDeviceToDevice, stream));
@@ -1795,7 +1800,14 @@ void Engine::getDeviceVector(const char *name, double *out)
     CUDA_OK(cudaMemcpy(out, d.upper, sizeof(double) * nm, cudaMemcpyDeviceToHost));
   else if (s == "cost")
     CUDA_OK(cudaMemcpy(out, d.cost, sizeof(double) * nm, cudaMemcpyDeviceToHost));
-  else if (s == "pivotVariable") {
+  else if (s == "primalDrift")
+    out[0] = lastPrimalDrift;
+  else if (s == "fake") {
+    std::vector<unsigned char> f(nm);
+    CUDA_OK(cudaMemcpy(f.data(), d.fake, nm, cudaMemcpyDeviceToHost));
+    for (int i = 0; i < nm; i++)
+      out[i] = f[i];
+  } else if (s == "pivotVariable") {
     std::vector<int> pv(m);
     CUDA_OK(cudaMemcpy(pv.data(), d.pivotVariable, sizeof(int) * m, cudaMemcpyDeviceToHost));
     for (int i = 0; i < m; i++)

@@ -136,6 +136,7 @@ public:
   void getWeights(double *w);
   void getDeviceVector(const char *name, double *out);
   int startup();                            // status -> basis, factorize, compute primals/duals
+  int refresh();                            // refactor + computeDuals + makeDualFeasible + computePrimals
 
   // ---- sensitivity analysis on the optimal basis the last dual() left on the device
   // (ClpSimplex::dualRanging / primalRanging, src/ClpSimplex.hpp:437,455 -> ClpSimplexOther.cpp:50,770;
@@ -219,7 +220,6 @@ private:
   void freeAll();
   int setupDevice();
   int refactor();          // factorize current basis (repairs singular bases)
-  int refresh();           // refactor + computeDuals + makeDualFeasible + computePrimals
   void enqueueIteration(bool timed, int slot);
   void enqueueBatchStart();
   void fetchState();

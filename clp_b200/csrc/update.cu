@@ -391,7 +391,8 @@ __global__ void permute_weights_kernel(const double *__restrict__ wOld, double *
     wNew[p] = srcPos[p] >= 0 ? wOld[srcPos[p]] : 1.0;
 }
 
-// dense nucleus gather: N[i][j] (row-major k x ld) = A[nucRow[i], nucCol[j]]
+// dense nucleus gather into a zeroed N: N[i][j] (row-major k x ld) = A[nucRow[i], nucCol[j]].  Entries of
+// a column that name the same row are added, as PRICE, times and S1 add them (loadProblem keeps them apart).
 __global__ void gather_nucleus_matrix_kernel(DeviceModel d, double *__restrict__ N, int ld)
 {
   const int lane = threadIdx.x & 31;
@@ -402,7 +403,7 @@ __global__ void gather_nucleus_matrix_kernel(DeviceModel d, double *__restrict__
   for (int e = d.colStart[col] + lane; e < d.colStart[col + 1]; e += 32) {
     int ni = d.posToNuc[d.rowIdx[e]];
     if (ni >= 0)
-      N[(size_t)ni * ld + j] = d.val[e];
+      atomicAdd(&N[(size_t)ni * ld + j], d.val[e]);
   }
 }
 

@@ -411,6 +411,7 @@ class ClpSimplex:
 
     def startup(self): return self._chk(self._L.Clpb_startup(self._h))
     def iterate(self, count): return self._chk(self._L.Clpb_iterate(self._h, int(count)))
+    def refresh(self): return self._chk(self._L.Clpb_refresh(self._h))
 
     def weights(self):
         w = np.zeros(self.numberRows())
@@ -420,7 +421,8 @@ class ClpSimplex:
     def deviceVector(self, name):
         n, m = self.numberColumns(), self.numberRows()
         size = {"sol": n + m, "dj": n + m, "rho": m, "alphaRow": n + m, "pivotVariable": m,
-                "status": n + m, "rhs3": 3 * m, "lower": n + m, "upper": n + m, "cost": n + m}[name]
+                "status": n + m, "rhs3": 3 * m, "lower": n + m, "upper": n + m, "cost": n + m, "fake": n + m,
+                "primalDrift": 1}[name]
         out = np.zeros(size)
         self._L.Clpb_getDeviceVector(self._h, name.encode(), _dp(out))
         return out

@@ -245,10 +245,18 @@ int Clpb_saveWeights(Clpb_Simplex *model, int mode);
    'count' iterations; DSE weights by pivot row (ClpDualRowSteepest::weights_) */
 int Clpb_startup(Clpb_Simplex *model);
 int Clpb_iterate(Clpb_Simplex *model, int count);
+/* ClpSimplexDual::statusOfProblemInDual (src/ClpSimplexDual.cpp:5024) on the device-resident state, as
+   dual() runs it at the end of every update cycle: refactorize the current basis (repairing a singular
+   one), recompute the duals, put every nonbasic variable on a dual feasible (where needed fake) bound,
+   recompute the basic values with one refinement step and measure their drift.  0, or -1 when no
+   factorizable basis was found. */
+int Clpb_refresh(Clpb_Simplex *model);
 void Clpb_getWeights(Clpb_Simplex *model, double *weights /* m */);
 /* debug reads of device vectors: "sol","dj" (n+m), "rho" (m), "alphaRow" (n+m),
    "pivotVariable" (m, as doubles), "status" (n+m, as doubles), the working bounds and costs
-   "lower","upper","cost" (n+m), and "rhs3" (3 x m): after Clpb_dualColumn / Clpb_dualColumnDevice
+   "lower","upper","cost" (n+m), "fake" (n+m, as doubles: 1 fake lower, 2 fake upper bound),
+   "primalDrift" (1: max_p |x - x_old| / (1 + |x|) over the basic values, of the last Clpb_refresh that
+   followed a factorization), and "rhs3" (3 x m): after Clpb_dualColumn / Clpb_dualColumnDevice
    the row pass's FTRAN right-hand sides [a_q, rho, flip column], after Clpb_updateWeights their
    FTRAN results [B^-1 a_q, B^-1 rho, B^-1 flip column] */
 void Clpb_getDeviceVector(Clpb_Simplex *model, const char *name, double *out);

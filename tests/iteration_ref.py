@@ -82,6 +82,27 @@ def solve_bound(x, kappa):
     return 1.0e-10 * (1.0 + np.abs(x).max(initial=0.0))
 
 
+class Worst:
+    """largest observed error / bound of every check (printed at the end of a test: pytest -s)"""
+
+    def __init__(self):
+        self.r = {}
+
+    def __call__(self, name, err, bound):
+        err, bound = np.asarray(err, dtype=np.float64).ravel(), np.asarray(bound, dtype=np.float64).ravel()
+        assert err.shape == bound.shape
+        bad = np.flatnonzero(~(err <= bound))
+        assert bad.size == 0, (name, bad[:8], err[bad[:8]], bound[bad[:8]])
+        if err.size:
+            i = int(np.argmax(err / np.maximum(bound, 1e-300)))
+            if err[i] / max(bound[i], 1e-300) >= self.r.get(name, (0.0,))[0]:
+                self.r[name] = (float(err[i] / max(bound[i], 1e-300)), float(err[i]), float(bound[i]))
+
+    def report(self, tag):
+        for k, (ratio, e, b) in sorted(self.r.items()):
+            print(f"[{tag}] {k}: worst error {e:.3g} (bound {b:.3g}, {ratio:.3g} of it)")
+
+
 # ---------------------------------------------------------------- CHUZR
 def chuzr(sol, lower, upper, weights, pivot_variable, tol=PRIMAL_TOL):
     """Dual steepest edge row choice of chuzr_key.  Returns (row, accepted rows): row is the packed-key argmax

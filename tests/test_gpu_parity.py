@@ -133,50 +133,6 @@ def test_unit_test_3x5_primals():
     np.testing.assert_allclose(sol[:5], [20.0 / 7.0, 3.0, 0.0, 0.0, 23.0 / 7.0], rtol=1e-12, atol=1e-12)
 
 
-@pytest.mark.parametrize("k", [1, 5, 31, 33, 100, 257, 700, 1500, 10400])
-def test_dense_invert(k):
-    """the dense LU + inverse of the refactorization (16-CTA cluster panel, TRSM, DGEMM).  At k = 10 400
-    the first five panels (10 400 ... 10 272 rows) are taller than the cluster's 16 x 640 rows and run on
-    the cooperative multi-CTA panel kernel, the rest on the cluster: both and the hand-over between them."""
-    rng = np.random.default_rng(k)
-    a = rng.standard_normal((k, k)) + np.diag(rng.uniform(0.5, 1.5, size=k) * np.sqrt(k) * rng.choice([-1, 1], size=k))
-    # make partial pivoting matter: shuffle rows
-    a = a[rng.permutation(k)]
-    info, x = clp_b200.denseInvert(a)
-    assert info == 0
-    if k <= 1500:
-        ref = np.linalg.inv(a)
-        np.testing.assert_allclose(x, ref, rtol=1e-9, atol=1e-9 * np.abs(ref).max())
-        res = np.abs(a @ x - np.eye(k)).max()
-    else:
-        # O(k^2) on the host: A (X E) - E for columns of I from the cooperative panels (< 160) and the end
-        cols = [0, 1, 31, 32, 100, 159, k - 33, k - 1]
-        e = np.zeros((k, len(cols)))
-        e[cols, np.arange(len(cols))] = 1.0
-        res = np.abs(a @ (x @ e) - e).max()
-    assert res < 1e-10 * k
-
-
-def _planted_singular_info(k, col):
-    rng = np.random.default_rng(0)
-    a = rng.standard_normal((k, k))
-    a[:, col] = a[:, 3] * 2.0 - a[:, 7]
-    info, _ = clp_b200.denseInvert(a)
-    return info
-
-
-def test_dense_invert_singular():
-    """a column that is a combination of two earlier ones is zero below the diagonal once they are
-    eliminated (rounding leaves ~1e-15, far below the 1e-11 pivot threshold): the LU reports exactly it"""
-    assert _planted_singular_info(64, 40) == 41
-
-
-def test_dense_invert_singular_in_cooperative_panel():
-    """the same at k = 10 400: column 100 lies in a panel of 10 304 rows, taller than the cluster kernel's
-    16 x 640, so the cooperative kernel finds it"""
-    assert _planted_singular_info(10400, 100) == 101
-
-
 # ------------------------------------------------------------------ ratio test
 def test_dual_column_against_oracle():
     lp = G.random_sparse_lp(200, 3000, 0.03, 21)

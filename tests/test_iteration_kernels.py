@@ -41,7 +41,7 @@ def engine(lp, **params):
     return s
 
 
-def conditioned_lp(m, n, k, seed, off=4):
+def conditioned_lp(m, n, k, seed, off=4, permute_homes=False):
     """An LP whose bases stay well conditioned.  Every column has one dominant entry of magnitude 10..20 on its
     home row and `off` entries U(-1, 1) on other rows, so a basis whose columns have distinct home rows is
     column-diagonally dominant (||B^-1||_1 <= 1).  Structurals 0..k-1 have home rows 0..k-1, the others a random
@@ -50,6 +50,8 @@ def conditioned_lp(m, n, k, seed, off=4):
     k..m-1 basic: a basis with a nucleus of exactly k."""
     rng = np.random.default_rng(seed)
     home = np.concatenate([np.arange(k), rng.integers(0, m, size=n - k)]) if m > 1 else np.zeros(n, dtype=np.int64)
+    if permute_homes:
+        home[:k] = np.random.default_rng([seed, k]).permutation(k)
     rows = np.empty((n, off + 1), dtype=np.int64)
     vals = np.empty((n, off + 1))
     rows[:, 0] = home
@@ -71,25 +73,14 @@ def conditioned_lp(m, n, k, seed, off=4):
     return lp, status
 
 
-class Worst:
-    """largest observed error / bound of every check (printed at the end of a test: pytest -s)"""
+def pivoting_lp(m, n, k, seed, off=4):
+    """conditioned_lp with the home rows of the k nucleus columns a random permutation of the nucleus rows: the
+    basis is as well conditioned, but the dominant entry of a nucleus column is off the diagonal, so the partial
+    pivoting of the refactorization interchanges in every panel."""
+    return conditioned_lp(m, n, k, seed, off, permute_homes=True)
 
-    def __init__(self):
-        self.r = {}
 
-    def __call__(self, name, err, bound):
-        err, bound = np.atleast_1d(np.asarray(err, dtype=np.float64)), np.atleast_1d(np.asarray(bound, dtype=np.float64))
-        assert err.shape == bound.shape
-        bad = np.flatnonzero(~(err <= bound))
-        assert bad.size == 0, (name, bad[:8], err[bad[:8]], bound[bad[:8]])
-        if err.size:
-            i = int(np.argmax(err / np.maximum(bound, 1e-300)))
-            if err[i] / max(bound[i], 1e-300) >= self.r.get(name, (0.0,))[0]:
-                self.r[name] = (float(err[i] / max(bound[i], 1e-300)), float(err[i]), float(bound[i]))
-
-    def report(self, tag):
-        for k, (ratio, e, b) in sorted(self.r.items()):
-            print(f"[{tag}] {k}: worst error {e:.3g} (bound {b:.3g}, {ratio:.3g} of it)")
+Worst = R.Worst
 
 
 def check_solve(worst, name, x, ref, kappa):
